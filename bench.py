@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of libuhdr_b200 (contract: see the task statement).
+"""bench.py -- headline benchmark of libuhdr_b200.
 
 Workload (BASELINE.json metric "MPix/s encode(API-1)+decode at 4K/8K"): one *step* = API-1 encode of
 a batch of F independent 3840x2160 frames (P010 HLG BT.2100 limited range + YUV420 BT.709, default
@@ -14,6 +14,10 @@ uhdr_get_encoded_stream).  Frames shard across ranks with no data-path collectiv
   e2e   : the same metric through the whole C-ABI sequence with HOST buffers every step (H2D of both
           inputs and D2H of the stream inside the timed region).
   extra : 8K decode (config 3) and 4K API-0 (config 2) device-resident numbers + applyGainMap roofline.
+
+`--dump-outputs DIR` writes what the timed loop's last step returned to the caller: the JPEG/R stream
+of three fixed frames (first, middle, last of rank 0's batch) as float32 byte values, and the stream
+size of every frame as float64.  Inputs are seeded, so two builds can be compared file by file.
 
 `--impl reference` times the reference's own CPU implementation (oracle/_ref: the reference sources
 compiled in place, its JPEG helper classes on the real libjpeg-turbo binary of this image) on all host
@@ -44,13 +48,13 @@ MPIX_4K = W4K * H4K / 1e6
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0}, "fallback"
+        return json.load(open(p)), "measured (MEASURED_PEAKS.json hbm_gbs)"
+    return {"hbm_gbs": 3350.0}, "H100 SXM data sheet, not measured"
 
 
 # ------------------------------------------------------------------------------------------------
 # synthetic frames: natural-image-like (smooth + texture) so the entropy coder sees realistic
-# statistics; every frame differs (phase shift) so a batch does not fit in L2 (8 x 37 MB > 126 MB)
+# statistics; every frame differs (phase shift) so a batch does not fit in L2 (8 x 37 MB > 50 MB)
 # ------------------------------------------------------------------------------------------------
 def make_frame(w, h, idx):
     yy, xx = np.mgrid[0:h, 0:w].astype(np.float32)
@@ -216,21 +220,12 @@ ALG_BYTES_PER_PX = {
     "apply_gainmap": 13.5,              # YUV420 1.5 + RGBA8888 map 4 read, RGBA-F16 8 written
     # SURVEY 8(d): FDCT+quant = 1 B/sample in + 2 B/sample out (4.5 B/px for 4:2:0, 9 B/px for 3-comp 4:4:4), avg of
     # the two launches.  The kernel is fused with the entropy coder's front end and writes 16 B per block instead
-    # of 128 B of coefficients, so its real DRAM traffic (roofline.traffic, ncu) is far below this figure.
+    # of 128 B of coefficients, so its real DRAM traffic is far below this figure.
     "fdct_quant": (4.5 + 9.0) / 2,
     # entropy coding proper: 16 B of block meta in (0.25 B/sample: 0.375 / 0.75 B/px) + the stream out (~0.28 B/px)
     "huff_encode": (0.375 + 0.75) / 2 + 0.28,
 }
 DATA_KERNELS = ("gainmap_pass1", "gainmap_affine", "fdct_quant", "huff_encode", "yuv_convert")
-
-
-def load_traffic():
-    """dram__bytes_read+write per launch from the committed ncu capture (profiles/), if any"""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:  # noqa: BLE001
-        return {}
 
 
 def nvml_handle(torch, local):
@@ -365,6 +360,8 @@ def bench_b200(args, rank, world):
     resident_steps(args.steps, open_timed_region)
     torch.cuda.synchronize()
     t_res = max_over_ranks(time.perf_counter() - clock["t0"])
+    if args.dump_outputs and rank == 0:
+        dump_streams(args.dump_outputs, lib, handles)
     l0 = clock["l0"]
     launches = lib.uhdr_b200_kernel_launches() - l0
     lib.uhdr_b200_set_kernel_timing(1)
@@ -506,7 +503,6 @@ def bench_b200(args, rank, world):
 
     pk, pk_kind = peaks()
     hbm = pk["hbm_gbs"]
-    traffic = load_traffic()
     kernels = {}
     for k, v in sorted(kt.items()):
         cnt, ms = v[:2]
@@ -524,10 +520,10 @@ def bench_b200(args, rank, world):
         name = max(cand)[1]
         e = kernels[name]
         roof = {"kernel": name, "bound": "hbm", "achieved": e["achieved_gbs"], "peak": hbm, "unit": "GB/s",
-                "frac": e["frac_of_hbm"], "traffic": traffic.get(name), "avg_launch_ms": e["avg_ms"],
+                "frac": e["frac_of_hbm"], "avg_launch_ms": e["avg_ms"],
                 "alg_bytes_per_launch": e["alg_bytes_per_launch"],
                 "share_of_step": round(kt[name][1] / sum(v[1] for v in kt.values()), 3),
-                "peak_kind": pk_kind + " (MEASURED_PEAKS.json hbm_gbs)",
+                "peak_kind": pk_kind,
                 "how": "CUDA events around every launch on its stream, %d steps with one encoder in flight" % args.steps}
 
     # single-GPU side measurements (config 2 / config 3 kernels, decode): N = 1 only
@@ -586,6 +582,19 @@ def bench_b200(args, rank, world):
     emit(line)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_streams(out_dir, lib, handles):
+    """the encoded streams the handles hold after the timed loop, as float32 byte values (< 64 MB in all)"""
+    os.makedirs(out_dir, exist_ok=True)
+    sizes = []
+    for i, hnd in enumerate(handles):
+        o = lib.uhdr_get_encoded_stream(hnd.h).contents
+        sizes.append(o.data_sz)
+        if i in (0, len(handles) // 2, len(handles) - 1):
+            data = np.frombuffer(C.string_at(o.data, o.data_sz), np.uint8)
+            np.save(os.path.join(out_dir, "stream_frame%02d.npy" % i), data.astype(np.float32))
+    np.save(os.path.join(out_dir, "stream_sizes.npy"), np.asarray(sizes, np.float64))
 
 
 def apply_8k(lib, hbm, iters=6):
@@ -865,15 +874,8 @@ def bench_reference(args, rank, world):
 
     def step():
         run_threads(conc, lambda i: api.encode(descs[i % len(descs)][0], descs[i % len(descs)][1]))
-    t0 = time.perf_counter()
-    step()            # also builds the reference's static LUTs
-    t_first = time.perf_counter() - t0
-    # keep the whole run within a few minutes whatever K and W the driver passes
+    step()            # the first warm-up step; also builds the reference's static LUTs
     steps, warmup = args.steps, args.warmup
-    budget = 150.0
-    if (steps + warmup) * t_first > budget:
-        warmup = min(warmup, 1)
-        steps = max(1, min(steps, int(budget / t_first) - warmup))
     for _ in range(max(0, warmup - 1)):
         step()
     # same rule as the GPU arm: the host threads walk the K steps back to back, no join between steps (a join
@@ -898,8 +900,7 @@ def bench_reference(args, rank, world):
         "impl": "reference", "metric": "MPix/s encode(API-1) at 4K", "value": round(v, 2), "unit": "MPix/s",
         "n_gpus": args.gpus, "steps": steps, "warmup": warmup, "ms_per_step": round(dt / steps * 1e3, 1),
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-        "config": {"workload": "api1_encode_3840x2160_p010hlg_bt2100+yuv420_bt709", "frames_per_step": per_step,
-                   "steps_requested": args.steps, "warmup_requested": args.warmup},
+        "config": {"workload": "api1_encode_3840x2160_p010hlg_bt2100+yuv420_bt709", "frames_per_step": per_step},
         "cpu_baseline": {"value": round(v, 2), "unit": "MPix/s", "cores": ncpu, "kind": "reference", "sample": sample},
         "e2e": {"value": round(v, 2), "unit": "MPix/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "decode": decode,
@@ -920,12 +921,18 @@ def emit(obj):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10,
+                    help="timed steps of the encode measurements (resident and end to end; --impl reference: the CPU "
+                         "arm); the 8K decode side measurement runs max(2, min(6, steps)) decodes per handle")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--frames", type=int, default=32, help="4K frames per GPU per step (config 4: 32 per GPU)")
     ap.add_argument("--slots", type=int, default=8, help="concurrent encoder handles (host threads) per GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's encoded streams (a fixed sample) as .npy files to DIR")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the library's outputs; it does not apply to --impl reference")
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     # stdout must carry exactly one JSON line: while the bench runs, file descriptor 1 points at

@@ -1,10 +1,10 @@
 /*
  * ultrahdr_api.h -- C ABI of libuhdr_b200, binary compatible with the reference's
- * /root/reference/ultrahdr_api.h (lib version 2.0.2): same enum values (:106-213), same POD
+ * ultrahdr_api.h (lib version 2.0.2): same enum values (:106-213), same POD
  * layouts (:220-283), same 43 exported entry points (:301-905).  An application compiled
  * against the reference header links against libuhdr_b200.so unchanged; the per-pixel work
  * (generateGainMap / applyGainMap / toneMap / convertYuv / JPEG DCT+quant+entropy stage) runs in
- * CUDA kernels on a B200 instead of the reference's CPU loops.
+ * CUDA kernels on an H100 (sm_90a) instead of the reference's CPU loops.
  *
  * Each declaration cites the reference line it replaces.
  */

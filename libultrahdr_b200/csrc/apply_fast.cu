@@ -13,8 +13,8 @@
 //     equals one packed hardware conversion per two channels (see pack_half4)
 //   * LUT indices come out of the float mantissa (add 2^23 toward zero) instead of the conversion unit
 // k_apply_lin1 (scale 1 -> linear half float, the 8K decode configuration) adds: a persistent grid
-// with atomic tile tickets, register prefetch of the next tile, packed fp32 pairs (packed_f32.cuh),
-// clamping on the packed half bit patterns and 256-bit stores; k_apply_fast covers the other
+// with atomic tile tickets, register prefetch of the next tile, fp32 pixel pairs (packed_f32.cuh),
+// clamping on the packed half bit patterns and two 128-bit stores per row; k_apply_fast covers the other
 // integer scales and the PQ / HLG outputs.
 #include <cuda_fp16.h>
 
@@ -252,14 +252,9 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyPara
 }
 
 // ---- scale 1, linear half-float output: the 8K decode configuration ----------------------------
-// Persistent grid (tables staged once per CTA, no wave tail) and packed-pair arithmetic: sm_100's
-// two-wide fp32 instructions (FMUL2 / FFMA2) work on the two horizontally adjacent pixels that
-// share a chroma sample, halving the issue slots of every multiply and add while each lane still
-// rounds exactly like the scalar instruction.  Only fused-multiply-add *forms* are written
-// (a*b + -0, a*1 + c, b*-1 + a): they equal the plain product / sum / difference bit for bit.
-// The -0 of the product form arrives as a kernel argument: with a literal the assembler reduces
-// the form to a multiply and then contracts it into a following add even though both carry .rn
-// (observed with ptxas 12.9), which would round once where the reference rounds twice.
+// Persistent grid (tables staged once per CTA, no wave tail); the two horizontally adjacent pixels
+// that share a chroma sample go through the arithmetic as a pair (packed_f32.cuh), each lane
+// rounding every step separately like the reference.  nz: the run-time -0 of the pair product.
 struct Lin1Smem {
   float srgb2[2048];
   float gain[768];
@@ -278,7 +273,7 @@ struct TileIn {   // what one thread reads for its 4x2 pixels
 
 template <int BPP, int GAMUT>
 __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyParams p, const float* __restrict__ gain_u8, const int tiles_x,
-                                                                 const int ntiles, const int wide_store, const unsigned long long nz,
+                                                                 const int ntiles, const unsigned long long nz,
                                                                  unsigned* __restrict__ sched) {
   __shared__ Lin1Smem sm;
   __shared__ int s_tile[4];
@@ -409,14 +404,8 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyP
         pack_half4_clamped(r1, g1, b1, out[4 * k + 2], out[4 * k + 3]);
       }
       uint2* d = (uint2*)p.dst + (size_t)(y + r) * p.dst_stride + x;
-      if (wide_store) {
-        asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(d), "r"(out[0]), "r"(out[1]), "r"(out[2]), "r"(out[3]),
-                     "r"(out[4]), "r"(out[5]), "r"(out[6]), "r"(out[7])
-                     : "memory");
-      } else {
-        ((uint4*)d)[0] = make_uint4(out[0], out[1], out[2], out[3]);
-        ((uint4*)d)[1] = make_uint4(out[4], out[5], out[6], out[7]);
-      }
+      ((uint4*)d)[0] = make_uint4(out[0], out[1], out[2], out[3]);
+      ((uint4*)d)[1] = make_uint4(out[4], out[5], out[6], out[7]);
     }
   };
   {
@@ -443,7 +432,6 @@ template <int BPP>
 cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sched, cudaStream_t s) {
   const int tiles_x = (p.sdr.w / 4 + kBlockX - 1) / kBlockX, tiles_y = (p.sdr.h + kBlockY * 2 - 1) / (kBlockY * 2);
   const int ntiles = tiles_x * tiles_y;
-  const int wide = (((size_t)p.dst & 31) == 0 && (p.dst_stride & 3) == 0) ? 1 : 0;
   dim3 block(kBlockX, kBlockY);
   const int g = p.gamut_identity ? 0 : (p.gamut_on_sdr ? 1 : 2);
   // persistent grid = exactly the CTAs that are co-resident (a partial second wave would double the time)
@@ -454,13 +442,13 @@ cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sc
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlockX * kBlockY, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident[g] = per_sm * (sms > 0 ? sms : 148);
+    resident[g] = per_sm * (sms > 0 ? sms : 132);
   }
   int ctas = resident[g];
   if (ctas > ntiles) ctas = ntiles;
-  if (g == 0) k_apply_lin1<BPP, 0><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, wide, kNegZero2, sched);
-  else if (g == 1) k_apply_lin1<BPP, 1><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, wide, kNegZero2, sched);
-  else k_apply_lin1<BPP, 2><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, wide, kNegZero2, sched);
+  if (g == 0) k_apply_lin1<BPP, 0><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  else if (g == 1) k_apply_lin1<BPP, 1><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  else k_apply_lin1<BPP, 2><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
   return cudaGetLastError();
 }
 

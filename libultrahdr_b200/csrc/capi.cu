@@ -1,5 +1,5 @@
 // The reference's public C API (ultrahdr_api.h:301-905, implemented in lib/src/ultrahdr_api.cpp)
-// on top of the B200 codec.  Same handle state machine: setters are rejected once the handle has
+// on top of the CUDA codec.  Same handle state machine: setters are rejected once the handle has
 // "sailed"; uhdr_encode / uhdr_decode are single shot and return their cached status when called
 // again; reset restores the defaults of ultrahdr_api.cpp:1452-1484 / 2045-2083.  Inputs are
 // uploaded to the device at set time (the reference deep-copies at the same point,
@@ -552,7 +552,7 @@ UHDR_API uhdr_error_info_t uhdr_enable_gpu_acceleration(uhdr_codec_private_t* co
 }
 static uhdr_error_info_t no_effects(uhdr_codec_private_t* codec) {
   if (!codec) return err(UHDR_CODEC_INVALID_PARAM, "received nullptr for uhdr codec instance");
-  return err(UHDR_CODEC_UNSUPPORTED_FEATURE, "image effects (editorhelper.cpp) are outside the B200 hot path");
+  return err(UHDR_CODEC_UNSUPPORTED_FEATURE, "image effects (editorhelper.cpp) are outside the CUDA hot path");
 }
 UHDR_API uhdr_error_info_t uhdr_add_effect_mirror(uhdr_codec_private_t* c, uhdr_mirror_direction_t) { return no_effects(c); }
 UHDR_API uhdr_error_info_t uhdr_add_effect_rotate(uhdr_codec_private_t* c, int) { return no_effects(c); }

@@ -307,7 +307,7 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
   const JpegFrame& f = h->frame;
   if (mode == 2) mode = f.ncomp == 1 ? 0 : 1;  // DECODE_STREAM :344-346
   if (h->adobe_transform == 0 && f.ncomp == 3)
-    return fail(E_UNSUPPORTED, "RGB (Adobe transform 0) JPEG input is not supported by the B200 decoder");
+    return fail(E_UNSUPPORTED, "RGB (Adobe transform 0) JPEG input is not supported by the CUDA decoder");
   if (mode == 1 && f.ncomp == 1) return fail(E_ERROR, "expected input color space to be JCS_YCbCr or JCS_RGB but got %d", 1);
   memset(out, 0, sizeof *out);
   out->cg = out->ct = -1;

@@ -1,5 +1,5 @@
 // The reference's C++ surface (include/ultrahdr/*.h: ultrahdr::UltraHdr, ultrahdr::JpegR incl. the
-// deprecated jr_* overloads, JpegEncoderHelper, JpegDecoderHelper) on top of the B200 codec.  The
+// deprecated jr_* overloads, JpegEncoderHelper, JpegDecoderHelper) on top of the CUDA codec.  The
 // classes are thin: arguments are validated like in the reference (error texts are its own), the work
 // is done by JpegRCodec / the engine stages on the calling thread's workspace (one stream + arenas per
 // host thread, created on first use).  Reference bodies: lib/src/jpegr.cpp:179-434 (encode API-0..4),

@@ -1,4 +1,4 @@
-// Host orchestration of the device stages: the B200 counterpart of the reference's
+// Host orchestration of the device stages: the CUDA counterpart of the reference's
 // UltraHdr::{generateGainMap, applyGainMap, toneMap, convertYuv} members
 // (lib/include/ultrahdr/ultrahdrcommon.h:471-546, bodies in lib/src/jpegr.cpp).  All functions
 // enqueue on the workspace stream and return without synchronising unless stated.

@@ -442,7 +442,7 @@ cudaError_t launch_fdct8(const Fdct8Params& Pin, cudaStream_t s) {
       oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fdct8<false>, 256, 0);
     }
     if (oe != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident = per_sm * (sms > 0 ? sms : 148);
+    resident = per_sm * (sms > 0 ? sms : 132);
   }
   if (code) {
     const int need = (total + 7) / 8;

@@ -537,7 +537,7 @@ int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_huff_encode, kEncThreads, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident = per_sm * (sms > 0 ? sms : 148);
+    resident = per_sm * (sms > 0 ? sms : 132);
   }
   int bpt = (int)((nblocks + (size_t)kEncThreads * resident - 1) / ((size_t)kEncThreads * resident));
   bpt = bpt < 1 ? 1 : (bpt > kMaxBpt ? kMaxBpt : bpt);

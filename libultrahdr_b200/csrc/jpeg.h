@@ -1,4 +1,4 @@
-// Baseline JPEG codec of libuhdr_b200: the B200 counterpart of JpegEncoderHelper /
+// Baseline JPEG codec of libuhdr_b200: the CUDA counterpart of JpegEncoderHelper /
 // JpegDecoderHelper (lib/src/jpegencoderhelper.cpp, lib/src/jpegdecoderhelper.cpp), which in the
 // reference are thin drivers over libjpeg-turbo.  Block arithmetic (colour conversion, level
 // shift, islow FDCT/IDCT, quantise/dequantise) runs in CUDA kernels; entropy coding runs on the device

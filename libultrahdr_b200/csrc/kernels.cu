@@ -1,4 +1,4 @@
-// Hand-written sm_100a kernels for the gain-map hot path.  Compile with -fmad=false: the
+// Hand-written sm_90a kernels for the gain-map hot path.  Compile with -fmad=false: the
 // reference CPU path is x86-64 baseline (SSE2, no FMA, lib CMakeLists.txt:290-301), so every
 // float expression below must round after each operation, in the reference's operand order.
 // Transcendentals are table fetches (tables.h) except where noted.  No tensor cores: this is

@@ -1,4 +1,4 @@
-// Device-side parameter blocks and launcher prototypes of the gain-map hot path (sm_100a).
+// Device-side parameter blocks and launcher prototypes of the gain-map hot path (sm_90a).
 // All launchers take DEVICE pointers and a stream; they never synchronise.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
 // Bit-exact device evaluation of glibc's powf (2.39, sysdeps/ieee754/flt-32/e_powf.c, the
-// x86-64 FMA multiarch variant the host CPUs of B200 boxes select).  Two sites of the reference
+// x86-64 FMA multiarch variant current x86-64 host CPUs select).  Two sites of the reference
 // call float std::pow on a *continuous* argument -- srgbOetf (gainmapmath.cpp:139-148, toneMap)
 // and hlgInverseOotfApprox (:303-306, HLG decode output) -- and their results feed 8/10-bit
 // quantisers, so a merely "correctly rounded" pow is not enough for bit-exact packed outputs:

@@ -38,12 +38,9 @@ def test_exports_every_declared_symbol(lib):
 
 
 def test_reference_symbol_list_is_covered(lib):
-    ref_hdr = "/root/reference/ultrahdr_api.h"
-    if not os.path.exists(ref_hdr):
-        pytest.skip("reference header not present on this box")
-    src = re.sub(r"/\*.*?\*/", "", open(ref_hdr).read(), flags=re.S)
-    src = "\n".join(l for l in src.split("\n") if not l.lstrip().startswith("#"))
-    names = set(re.findall(r"UHDR_EXTERN[^;(]*?\b(\w+)\s*\(", src))
+    # the UHDR_EXTERN functions of the reference's ultrahdr_api.h (lib version 2.0.2), one per line
+    with open(os.path.join(os.path.dirname(__file__), "golden", "ref_api_symbols.txt")) as f:
+        names = set(f.read().split())
     assert len(names) == 43
     assert not [n for n in names if not hasattr(lib, n)]
 

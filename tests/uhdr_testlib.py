@@ -26,7 +26,6 @@ REF_TURBO_SO = os.path.join(ROOT, "oracle", "_ref", "libuhdr_ref_turbo.so")
 REF_SO = REF_TURBO_SO if os.path.exists(REF_TURBO_SO) else REF_SHIM_SO
 ORACLE_SO = os.path.join(ROOT, "oracle", "liboracle.so")
 GPU_SO = os.environ.get("UHDR_B200_SO") or os.path.join(ROOT, "libultrahdr_b200", "libuhdr_b200.so")
-REF_DATA = "/root/reference/tests/data"
 SEED = 20240607
 
 
@@ -118,13 +117,6 @@ def make_rgbaf16(w, h, seed=SEED + 3):
 def make_rgba8888(w, h, seed=SEED + 4):
     rs = np.random.RandomState(seed)
     return (rs.randint(0, 1 << 24, w * h).astype(np.uint32) | np.uint32(0xFF000000))
-
-
-def load_fixture_720p():
-    """config 1 inputs; only available in the build container (not on the GPU box)."""
-    p = np.fromfile(os.path.join(REF_DATA, "raw_p010_image.p010"), dtype=np.uint16)
-    y = np.fromfile(os.path.join(REF_DATA, "raw_yuv420_image.yuv420"), dtype=np.uint8)
-    return p, y
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1,8 +1,8 @@
-"""Generates tests/golden/uhdr_golden_320x192.npz in the BUILD container: a 320x192 crop of the
-reference's own 1280x720 fixtures (tests/data/raw_p010_image.p010 + raw_yuv420_image.yuv420, the
-config-1 inputs) together with the outputs of the reference's own code (oracle/_ref, compiled from
-/root/reference in place) for every stage of the hot path.  The GPU box has neither
-/root/reference nor its fixtures; these vectors travel with the repo instead."""
+"""Generates tests/golden/uhdr_golden_320x192.npz: a 320x192 crop of the reference's own 1280x720
+fixtures (tests/data/raw_p010_image.p010 + raw_yuv420_image.yuv420, the config-1 inputs) together with
+the outputs of the reference's own code (oracle/_ref) for every stage of the hot path, so that the tests
+need neither the reference checkout nor its fixtures.
+    python tools/make_golden.py /path/to/libultrahdr"""
 import os
 import sys
 
@@ -15,7 +15,8 @@ import uhdr_testlib as T  # noqa: E402
 from libultrahdr_b200 import ctypes_api as A  # noqa: E402
 
 W, H, X0, Y0, CW, CH = 1280, 720, 864, 312, 320, 192  # most varied 320x192 window of the colour-bar fixture
-p010, yuv = T.load_fixture_720p()
+p010 = np.fromfile(os.path.join(sys.argv[1], "tests", "data", "raw_p010_image.p010"), dtype=np.uint16)
+yuv = np.fromfile(os.path.join(sys.argv[1], "tests", "data", "raw_yuv420_image.yuv420"), dtype=np.uint8)
 Y = p010[:W * H].reshape(H, W)[Y0:Y0 + CH, X0:X0 + CW]
 UV = p010[W * H:].reshape(H // 2, W)[Y0 // 2:(Y0 + CH) // 2, X0:X0 + CW]
 hb = np.concatenate([Y.ravel(), UV.ravel()]).astype(np.uint16)
