@@ -99,7 +99,8 @@ UHDR_EXTERN int uhdr_b200_enc_rearm(uhdr_codec_private_t* enc);
 UHDR_EXTERN size_t uhdr_b200_trim_cache(void);
 /* Where JpegDecoderHelper's entropy decoding (libjpeg-turbo jdhuff.c behind jpegdecoderhelper.cpp:397-411)
  * runs: 0 (default) and 2 = on the device for every stream the parallel decoder accepts, whatever its size (the
- * host decoder only takes the streams it declines: restart markers, no fixed point, inconsistent data);
+ * host decoder only takes the streams it declines: restart markers out of sequence or in the wrong number, RST markers
+ * without a DRI marker, another marker before EOI, no fixed point, inconsistent data);
  * 1 = host, for tests and triage.  Process-wide; returns the previous setting.  Results are identical either way. */
 UHDR_EXTERN int uhdr_b200_set_entropy_decoder(int mode);
 /* out[0] = scans entropy-decoded on the device so far, out[1] = scans the device decoder handed back to
