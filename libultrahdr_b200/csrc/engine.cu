@@ -210,11 +210,10 @@ int generate_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& hdr
       TIMED(ws, "gainmap_onepass", launch_gainmap_onepass(p, ws.stream()));
     return E_OK;
   }
-  p.gains = (float*)ws.dalloc(sizeof(float) * (size_t)mw * mh * p.nch);
   p.minmax = (unsigned*)ws.dalloc(128);
   float* d_minmax_f = (float*)ws.dalloc(64);
   job->h_minmax = (float*)ws.halloc(64);
-  if (!p.gains || !p.minmax || !d_minmax_f || !job->h_minmax) return E_MEM;
+  if (!p.minmax || !d_minmax_f || !job->h_minmax) return E_MEM;
   GainmapFinalizeParams f;
   f.minmax = p.minmax;
   f.minmax_f = d_minmax_f;
@@ -223,6 +222,28 @@ int generate_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& hdr
   f.has_user_min = cfg.min_content_boost != FLT_MIN;
   f.log2_user_max = f.has_user_max ? std::log2(cfg.max_content_boost) : 0.0f;
   f.log2_user_min = f.has_user_min ? std::log2(cfg.min_content_boost) : 0.0f;
+  // Two-pass on the fast kernels.  Scale 1: a statistics pass leaves only the extremes of the quotient (hdr+eps)/(sdr+eps)
+  // per class (dark or not), and a code pass recomputes every quotient and maps it to its byte, taking the log2 in fp32
+  // wherever the byte provably does not depend on more.  Scales 2 / 4: the float plane carries the quotient (sign = dark
+  // pixel) to k_affine_q.  UHDR_B200_GAINS_PLANE=1 keeps the log2 in pass 1 and a plane of gains (measurement / triage).
+  static const bool keep_gains_plane = getenv("UHDR_B200_GAINS_PLANE") != nullptr;
+  job->exact_word = nullptr;
+  p.gamma = cfg.gamma;
+  // the code pass stores bytes like the one-pass kernel: gamma 1 and its conditions on dst
+  const bool q2 = p.scale == 1 && !keep_gains_plane && gainmap_fast_eligible(p, true);
+  if (q2) {
+    CUDA_TRY(launch_init_q_keys(p.minmax, ws.stream()));
+    // words 8 and 10: tile tickets of the two passes, 9: exact-path count (all zeroed by init_q_keys)
+    TIMED(ws, "gainmap_pass1", launch_gainmap_q2(p, f, false, p.minmax + 8, nullptr, ws.stream()));
+    TIMED(ws, "gainmap_affine", launch_gainmap_q2(p, f, true, p.minmax + 10, p.minmax + 9, ws.stream()));
+    job->exact_word = reinterpret_cast<unsigned*>(job->h_minmax + 8);
+    job->values = (unsigned long long)mw * mh * p.nch;
+    CUDA_TRY(cudaMemcpyAsync(job->exact_word, p.minmax + 9, sizeof(unsigned), cudaMemcpyDeviceToHost, ws.stream()));
+    CUDA_TRY(cudaMemcpyAsync(job->h_minmax, d_minmax_f, 6 * sizeof(float), cudaMemcpyDeviceToHost, ws.stream()));
+    return E_OK;
+  }
+  p.gains = (float*)ws.dalloc(sizeof(float) * (size_t)mw * mh * p.nch);
+  if (!p.gains) return E_MEM;
   AffineParams a;
   a.gains = p.gains;
   a.minmax_f = d_minmax_f;
@@ -232,13 +253,8 @@ int generate_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& hdr
   a.nch = p.nch;
   a.dst_stride = p.dst_stride;
   a.gamma = cfg.gamma;
-  // Both passes on their fast kernels: the float plane carries the quotient (sign = dark pixel) and pass 2 takes the
-  // log2 -- in fp32 wherever the byte provably does not depend on more (k_affine_q).  UHDR_B200_GAINS_PLANE=1 keeps
-  // the log2 in pass 1 (measurement / triage).
-  static const bool keep_gains_plane = getenv("UHDR_B200_GAINS_PLANE") != nullptr;
   const bool pass1_fast = gainmap_fast_eligible(p, false), affine_fast = affine_fast_eligible(a);
-  const bool q_mode = pass1_fast && affine_fast && !keep_gains_plane;
-  job->exact_word = nullptr;
+  const bool q_mode = p.scale != 1 && pass1_fast && affine_fast && !keep_gains_plane;
   if (q_mode) {
     p.store_q = 1;
     CUDA_TRY(launch_init_q_keys(p.minmax, ws.stream()));

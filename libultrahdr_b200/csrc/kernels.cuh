@@ -36,8 +36,8 @@ struct GainmapGenParams {  // generateGainMap, lib/src/jpegr.cpp:530-1058
   // one-pass fast kernels: correctly rounded 1 / double(log2_max - log2_min), or 0 when that range is zero / not finite
   // (then the kernels divide); see encode_gain_norm in gainmap_fast.cu
   double inv_log2_range;
-  // two-pass fast kernels: the float plane receives the quotient (hdr+eps)/(sdr+eps) per value, negated when the
-  // pixel is dark (sdr < 2/255), instead of its log2; minmax holds q keys (k_affine_q finishes the job)
+  // two-pass fast kernels at map scale 2 / 4: the float plane receives the quotient (hdr+eps)/(sdr+eps) per value,
+  // negated when the pixel is dark (sdr < 2/255), instead of its log2; minmax holds q keys (k_affine_q finishes the job)
   int store_q;
   uint8_t* dst;                     // RGB888 / Y400
   int dst_stride;                   // pixels
@@ -180,6 +180,11 @@ cudaError_t launch_pow_fast_probe(unsigned first_bits, unsigned count, float* d_
 void tonemap_screen_stats(unsigned long long out[2]);
 bool gainmap_fast_eligible(const GainmapGenParams& p, bool onepass);
 cudaError_t launch_gainmap_fast(const GainmapGenParams& p, bool onepass, unsigned* sched, cudaStream_t s);
+// two-pass map at scale 1 without a plane, keys set up by launch_init_q_keys: the statistics pass (code = false) leaves
+// the extremes of the quotient in p.minmax; the code pass (code = true) recomputes every quotient and writes its byte to
+// p.dst, fin.minmax_f and the exact-path count.  sched: a zeroed tile-ticket word per pass.
+cudaError_t launch_gainmap_q2(const GainmapGenParams& p, const GainmapFinalizeParams& fin, bool code, unsigned* sched,
+                              unsigned* exact_count, cudaStream_t s);
 cudaError_t launch_log2_probe(const float* d_in, float* d_out, int n, cudaStream_t s);
 cudaError_t launch_powf_probe(const float* d_in, float y, float* d_out, int n, cudaStream_t s);
 cudaError_t launch_tonemap(const TonemapParams& p, cudaStream_t s);
