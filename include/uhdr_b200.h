@@ -106,8 +106,11 @@ UHDR_EXTERN int uhdr_b200_set_entropy_decoder(int mode);
 /* out[0] = scans entropy-decoded on the device so far, out[1] = scans the device decoder handed back to
  * the host decoder, out[2] = relaxation rounds the last device decode needed */
 UHDR_EXTERN void uhdr_b200_entropy_decoder_stats(unsigned long long out[3]);
-/* Two-pass generateGainMap on the fast kernels keeps the quotient (hdr+eps)/(sdr+eps) in its float plane and takes the
- * log2 in pass 2, in fp32 (lg2.approx) wherever the output byte provably does not depend on more, in fp64 otherwise.
+/* Two-pass generateGainMap with gamma 1 on the fast kernels takes the log2 of the quotient (hdr+eps)/(sdr+eps) only
+ * when it maps the quotient to its byte: in fp32 (lg2.approx) wherever the byte provably does not depend on more, in
+ * fp64 otherwise.  At map scale 1 a statistics pass finds the extremes of the quotient and a code pass recomputes every
+ * quotient and writes its byte; at scales 2 / 4 a float plane carries the quotients to the byte pass.  Other routes
+ * (gamma != 1, the generic kernels, UHDR_B200_GAINS_PLANE) do not count here.
  * out[0] = gain values quantised that way since process start, out[1] = how many of them took the fp64 path. */
 UHDR_EXTERN void uhdr_b200_generate_stats(unsigned long long out[2]);
 /* diagnostic: worst[0] = max over the `count` floats whose bit patterns start at first_bits of

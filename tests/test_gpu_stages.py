@@ -96,7 +96,8 @@ def test_generate_rgba8888_sdr_and_boost_hints(gpu, checker):
 
 
 def test_generate_fast_path_hints_and_degenerate_ranges(gpu, checker):
-    """The quotient-plane two-pass path (P010 + YUV420) with content-boost hints (they clamp min / max after the
+    """The fast two-pass path (P010 + YUV420: statistics + code pass at scale 1, quotient plane at scale 4) with
+    content-boost hints (they clamp min / max after the
     extremes were found, which makes the affine range small and many values saturate), with constant images (range
     forced to 0.1 by the |max - min| < eps rule), with an all-dark SDR image (only the capped class exists), at
     scales 1 / 4 and both channel counts."""
@@ -371,8 +372,8 @@ def test_fast_log2_error_bound(gpu):
 
 
 def test_two_pass_takes_the_exact_log2_only_near_byte_boundaries(gpu, checker):
-    """k_affine_q's screen: on noise (every gain value different) a small share of the values takes the fp64 path,
-    and the map is still bit exact (the other tests); on a constant image none has to."""
+    """The lg2.approx screen of the scale-1 code pass (affine_q_pair, shared with k_affine_q): on noise (every gain
+    value different) a small share of the values takes the fp64 path, and the map is still bit exact."""
     lib = gpu.lib
 
     def stats():
@@ -387,7 +388,7 @@ def test_two_pass_takes_the_exact_log2_only_near_byte_boundaries(gpu, checker):
     v1, e1 = stats()
     g2, m2 = checker.generate(sdr, hdr)
     assert (g1 == g2).all() and T.md_equal(m1, m2)
-    assert v1 - v0 == w * h * 3, "the quotient-plane path did not run"
+    assert v1 - v0 == w * h * 3, "the statistics + code pass did not run"
     share = (e1 - e0) / float(v1 - v0)
     assert 0.0 < share < 0.02, share
 

@@ -89,6 +89,31 @@ def test_generate_other_formats_and_options(pair):
             assert (g1 == g2).all() and T.md_equal(m1, m2), (hfmt, kw)
 
 
+def test_code_lattice(pair):
+    """Every HDR and SDR luma code with full-range chroma (uhdr_testlib.make_code_lattice), with clean and dirty
+    P010 low bits: limited-range codes outside 64..940 drive the normalised values below 0 and above 1, where the
+    clamps and table indices have to agree.  generateGainMap over range, transfer, channels, scale and preset,
+    and toneMap on the same HDR frames."""
+    R, O = pair
+    w, h = 1024, 256
+    bad = []
+    for dirty in (False, True):
+        hb, sb = T.make_code_lattice(w, h, dirty)
+        sdr, k2 = A.yuv420_image(sb, w, h, A.CG_BT709)
+        for rng, ct in itertools.product([A.CR_LIMITED, A.CR_FULL], [A.CT_HLG, A.CT_PQ]):
+            hdr, k1 = A.p010_image(hb, w, h, A.CG_BT2100, ct, rng)
+            for multi, scale, preset in itertools.product([0, 1], [1, 4], [0, 1]):
+                cfg = A.default_gm_config(scale_factor=scale, multichannel=multi, preset=preset)
+                g1, m1 = R.generate(sdr, hdr, cfg)
+                g2, m2 = O.generate(sdr, hdr, cfg)
+                if not ((g1 == g2).all() and T.md_equal(m1, m2)):
+                    bad.append(("generate", dirty, rng, ct, multi, scale, preset, int((g1 != g2).sum())))
+            a, b = R.tonemap(hdr)[0], O.tonemap(hdr)[0]
+            if not (a == b).all():
+                bad.append(("tonemap", dirty, rng, ct, int((a != b).sum())))
+    assert not bad, bad
+
+
 def test_apply_matrix(pair):
     R, O = pair
     for multi, scale in ((1, 1), (0, 1), (1, 4), (0, 2)):

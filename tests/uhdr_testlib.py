@@ -96,6 +96,22 @@ def make_yuv420(w, h, kind="noise", seed=SEED + 1):
     raise ValueError(kind)
 
 
+def make_code_lattice(w=1024, h=256, dirty=False, seed=SEED + 5):
+    """Every input code: HDR luma code = x % 1024 (all of 0..1023 in each row of a 1024-wide frame), SDR luma =
+    y % 256, seeded random chroma over the whole 10-bit / 8-bit range.  Limited-range codes below 64 and above
+    940 / 960 are legal inputs too.  dirty: random values 0..63 in the low 6 bits of every P010 word, which
+    the reference ignores (getP010Pixel shifts them out).  -> (p010 uint16, yuv420 uint8)"""
+    rs = np.random.RandomState(seed)
+    yy, xx = np.mgrid[0:h, 0:w]
+    huv = rs.randint(0, 1024, (h // 2) * w)
+    suv = rs.randint(0, 256, 2 * (w // 2) * (h // 2))
+    p010 = np.concatenate([(xx % 1024).ravel(), huv]).astype(np.uint16) << 6
+    if dirty:
+        p010 |= rs.randint(0, 64, p010.size).astype(np.uint16)
+    yuv = np.concatenate([(yy % 256).ravel(), suv]).astype(np.uint8)
+    return np.ascontiguousarray(p010), np.ascontiguousarray(yuv)
+
+
 def make_rgba1010102(w, h, seed=SEED + 2):
     rs = np.random.RandomState(seed)
     return (rs.randint(0, 1 << 30, w * h).astype(np.uint32) | np.uint32(3 << 30))
