@@ -121,6 +121,11 @@ UHDR_EXTERN int uhdr_b200_probe_log2_fast(unsigned first_bits, unsigned count, f
  * redone with the exact routine only if one of its six 8-bit codes could depend on the difference.
  * out[0] = groups processed since process start, out[1] = groups redone (current device). */
 UHDR_EXTERN void uhdr_b200_tonemap_stats(unsigned long long out[2]);
+/* applyGainMap kernel launches since process start, every entry point (host buffers, device pointers, the C++
+ * surface, uhdr_decode): out[0] = k_apply_lin1 (scale 1 -> linear half float), out[1] = k_apply_fast (other integer
+ * scales up to 16 and the PQ / HLG outputs), out[2] = k_apply_gainmap (every other input), out[3] = gain-map resizes
+ * (aspect ratio off by more than 1 %), each followed by one of the other three. */
+UHDR_EXTERN void uhdr_b200_apply_stats(unsigned long long out[4]);
 /* diagnostic: worst[0] = max |approximate pow(e, 1/2.4) - the exact one| over the `count` floats whose bit patterns
  * start at first_bits (the screen relies on <= 3e-7 for e in (0.0031308, 1]; must measure <= 1.5e-7); host pointer. */
 UHDR_EXTERN int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst);

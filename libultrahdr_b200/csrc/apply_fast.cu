@@ -42,11 +42,24 @@ __device__ __forceinline__ void pack_half4(float r, float g, float b, unsigned& 
   hi = *reinterpret_cast<const unsigned*>(&ba);
 }
 
-// kMaxH = reference floatToHalf(10000/203) = 0x5228; the alpha half 0x3C00 passes through both bounds
+// `mask` if x is a NaN, else 0.  A NaN channel occurs with valid metadata: a max_content_boost of FLT_MAX
+// puts +inf into the gain table, and then 0 * inf (black base pixel, offset 0) or inf - inf (a gamut row)
+// is NaN.  The reference's clamps are comparisons, which keep the NaN, x86 makes it the default NaN
+// 0xFFC00000, and floatToHalf of that is 0xFFFF: ORing the mask into a clamped half writes the same.
+__device__ __forceinline__ unsigned nan_bits(float x, unsigned mask) { return x != x ? mask : 0u; }
+
+// kMaxH = reference floatToHalf(10000/203) = 0x5228; the alpha half 0x3C00 passes through both bounds.
+// The conversion turns NaN and +-inf alike into a NaN half (bits | 1), so NaN is told apart on the floats;
+// NANS = false where the host has ruled out inf and NaN (ApplyParams::nan_possible), which saves the selects.
+template <bool NANS>
 __device__ __forceinline__ void pack_half4_clamped(float r, float g, float b, unsigned& lo, unsigned& hi) {
   pack_half4(r, g, b, lo, hi);
   lo = __vmins2(__vmaxs2(lo, 0u), 0x52285228u);
   hi = __vmins2(__vmaxs2(hi, 0u), 0x52285228u);
+  if (NANS) {
+    lo |= nan_bits(r, 0xFFFFu) | nan_bits(g, 0xFFFF0000u);
+    hi |= nan_bits(b, 0xFFFFu);
+  }
 }
 
 // Shared-memory tables, byte-offset addressed.
@@ -195,13 +208,17 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyPara
           const float c = p.gamut[6] * hr + p.gamut[7] * hg + p.gamut[8] * hb;
           hr = a; hg = b; hb = c;
         }
-        // clampPixelFloatLinear; min/max form is equivalent here: no NaN and no negative zero can
-        // reach this point (sums of a positive-leading gamut row, x - x == +0)
+        // clampPixelFloatLinear; the min/max form equals it for numbers (no negative zero reaches this
+        // point: sums of a positive-leading gamut row, x - x == +0), but drops a NaN, which the reference
+        // keeps: a NaN channel is written as the reference's 0xFFFF (nan_bits)
+        const unsigned nan_lo = nan_bits(hr, 0xFFFFu) | nan_bits(hg, 0xFFFF0000u), nan_hi = nan_bits(hb, 0xFFFFu);
         const float kMax = 10000.0f / 203.0f;
         hr = fminf(fmaxf(hr, 0.0f), kMax);
         hg = fminf(fmaxf(hg, 0.0f), kMax);
         hb = fminf(fmaxf(hb, 0.0f), kMax);
         pack_half4(hr, hg, hb, out[2 * i], out[2 * i + 1]);
+        out[2 * i] |= nan_lo;
+        out[2 * i + 1] |= nan_hi;
       } else {
         hr = hr * 203.0f / p.out_nits;
         hg = hg * 203.0f / p.out_nits;
@@ -271,7 +288,7 @@ struct TileIn {   // what one thread reads for its 4x2 pixels
   int x, y;
 };
 
-template <int BPP, int GAMUT>
+template <int BPP, int GAMUT, bool NANS>
 __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyParams p, const float* __restrict__ gain_u8, const int tiles_x,
                                                                  const int ntiles, const unsigned long long nz,
                                                                  unsigned* __restrict__ sched) {
@@ -400,8 +417,8 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyP
         // their last mantissa bit as well is harmless.
         float r0, r1, g0, g1, b0, b1;
         un(hr, r0, r1); un(hg, g0, g1); un(hb, b0, b1);
-        pack_half4_clamped(r0, g0, b0, out[4 * k], out[4 * k + 1]);
-        pack_half4_clamped(r1, g1, b1, out[4 * k + 2], out[4 * k + 3]);
+        pack_half4_clamped<NANS>(r0, g0, b0, out[4 * k], out[4 * k + 1]);
+        pack_half4_clamped<NANS>(r1, g1, b1, out[4 * k + 2], out[4 * k + 3]);
       }
       uint2* d = (uint2*)p.dst + (size_t)(y + r) * p.dst_stride + x;
       ((uint4*)d)[0] = make_uint4(out[0], out[1], out[2], out[3]);
@@ -428,7 +445,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyP
   }
 }
 
-template <int BPP>
+template <int BPP, bool NANS>
 cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sched, cudaStream_t s) {
   const int tiles_x = (p.sdr.w / 4 + kBlockX - 1) / kBlockX, tiles_y = (p.sdr.h + kBlockY * 2 - 1) / (kBlockY * 2);
   const int ntiles = tiles_x * tiles_y;
@@ -438,7 +455,8 @@ cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sc
   static int resident[3] = {0, 0, 0};
   if (!resident[g]) {
     int per_sm = 0, dev = 0, sms = 0;
-    const void* fn = g == 0 ? (const void*)k_apply_lin1<BPP, 0> : g == 1 ? (const void*)k_apply_lin1<BPP, 1> : (const void*)k_apply_lin1<BPP, 2>;
+    const void* fn = g == 0 ? (const void*)k_apply_lin1<BPP, 0, NANS> : g == 1 ? (const void*)k_apply_lin1<BPP, 1, NANS>
+                                                                         : (const void*)k_apply_lin1<BPP, 2, NANS>;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlockX * kBlockY, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
@@ -446,10 +464,14 @@ cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sc
   }
   int ctas = resident[g];
   if (ctas > ntiles) ctas = ntiles;
-  if (g == 0) k_apply_lin1<BPP, 0><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
-  else if (g == 1) k_apply_lin1<BPP, 1><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
-  else k_apply_lin1<BPP, 2><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  if (g == 0) k_apply_lin1<BPP, 0, NANS><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  else if (g == 1) k_apply_lin1<BPP, 1, NANS><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  else k_apply_lin1<BPP, 2, NANS><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
   return cudaGetLastError();
+}
+template <int BPP>
+cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sched, cudaStream_t s) {
+  return p.nan_possible ? launch_lin1<BPP, true>(p, gain_u8, sched, s) : launch_lin1<BPP, false>(p, gain_u8, sched, s);
 }
 
 template <int BPP, bool S1, int G>

@@ -1,10 +1,13 @@
 #include "engine.h"
 
+#include <algorithm>
 #include <atomic>
 #include <cfloat>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+
+#include "container.h"
 
 namespace uhdr_b200 {
 
@@ -320,6 +323,14 @@ void finish_gainmap_metadata(const GainmapJob& job, uhdr_gainmap_metadata_t* md)
 }
 
 // ------------------------------------------------------------------------------------------------
+namespace {
+// applyGainMap launches since process start: k_apply_lin1, k_apply_fast, k_apply_gainmap, k_resize_map
+std::atomic<unsigned long long> g_apply_routes[4];
+}  // namespace
+void apply_route_stats(unsigned long long out[4]) {
+  for (int i = 0; i < 4; i++) out[i] = g_apply_routes[i].load(std::memory_order_relaxed);
+}
+
 int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in,
                       const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                       DevImage* dst) {
@@ -334,6 +345,9 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
                 "{UHDR_CT_LINEAR, UHDR_CT_HLG, UHDR_CT_PQ}. Received %d", out_ct);
   if ((out_ct == UHDR_CT_LINEAR && dst->v.fmt != F_RGBAF16) || (out_ct != UHDR_CT_LINEAR && dst->v.fmt != F_RGBA1010102))
     return fail(E_INVALID_PARAM, "unsupported destination pixel format %d for output color transfer %d", dst->v.fmt, out_ct);
+  // :1585 uhdr_validate_gainmap_metadata_descriptor.  The kernels rely on it: hdr_capacity_max == hdr_capacity_min
+  // gives a NaN weight, and gamma < 0 an infinite gain-LUT input whose table index overflows
+  if (int rc = validate_metadata(md)) return rc;
   if (sdr.v.fmt != F_YUV444 && sdr.v.fmt != F_YUV422 && sdr.v.fmt != F_YUV420 && sdr.v.fmt != F_RGB888 && sdr.v.fmt != F_RGBA8888)
     return fail(E_UNSUPPORTED, "apply gainmap method expects base image color format to be one of "
                 "{YCbCr444, YCbCr422, YCbCr420, RGB888, RGBA8888}. Received %d", sdr.v.fmt);
@@ -364,6 +378,7 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
       r.dst = (uint8_t*)rs.v.p[0];
       r.dst_w = sdr.v.w; r.dst_h = sdr.v.h; r.dst_stride = rs.v.stride[0];
       TIMED(ws, "resize_gainmap", launch_resize_map(r, ws.stream()));
+      g_apply_routes[3].fetch_add(1, std::memory_order_relaxed);
       rs.cg = map.cg; rs.ct = map.ct; rs.range = map.range;
       map = rs;
     }
@@ -412,10 +427,18 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
   p.gain_lut = d_tab;
   p.idw = d_tab + 3 * 1024;
   const bool single = metadata_single_channel(m);
+  double max_off = 0.0;
   for (int c = 0; c < 3; c++) {
     p.gamma_inv[c] = 1.0f / md.gamma[single ? 0 : c];
     p.off_sdr[c] = md.offset_sdr[c];
     p.off_hdr[c] = md.offset_hdr[c];
+    max_off = std::max(max_off, (double)md.offset_sdr[c]);
+  }
+  {  // a channel is (linear base + offset) * factor - offset, then a gamut row (sum of |coefficients| < 2.4), with
+     // the linear base <= 1: below FLT_MAX / 4 nothing overflows, and without inf no NaN (0 * inf, inf - inf) occurs
+    double max_f = 0.0;
+    for (int i = 0; i < 3 * 1024; i++) max_f = std::max(max_f, (double)h_tab[i]);
+    p.nan_possible = !(max_f * (1.0 + max_off) * 4.0 < (double)FLT_MAX);
   }
   yuv2rgb_coeffs(UHDR_CG_DISPLAY_P3, p.y2r);
   p.sdr = sdr.v;
@@ -430,10 +453,13 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
   p.luts = ws.luts();
   p.dst = (void*)dst->v.p[0];
   p.dst_stride = dst->v.stride[0];
-  if (apply_fast_eligible(p))
+  if (apply_fast_eligible(p)) {
     TIMED(ws, "apply_gainmap", launch_apply_fast(p, d_tab + 3 * 1024 + idw_floats, ws.stream()));
-  else
+    g_apply_routes[p.scale_int == 1 && out_ct == UHDR_CT_LINEAR ? 0 : 1].fetch_add(1, std::memory_order_relaxed);
+  } else {
     TIMED(ws, "apply_gainmap", launch_apply_gainmap(p, ws.stream()));
+    g_apply_routes[2].fetch_add(1, std::memory_order_relaxed);
+  }
   return E_OK;
 }
 

@@ -45,6 +45,8 @@ void gainmap_affine_stats(unsigned long long out[2]);
 int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map,
                       const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                       DevImage* dst /* allocated by caller, fmt F16 / 1010102 */);
+// apply_gainmap_dev launches since process start: [0] k_apply_lin1, [1] k_apply_fast, [2] k_apply_gainmap, [3] k_resize_map
+void apply_route_stats(unsigned long long out[4]);
 int tonemap_dev(Workspace& ws, const DevImage& hdr, DevImage* sdr /* allocated by caller */);
 // in_place = false: the result goes to workspace scratch and *img is redirected to it (the source stays intact)
 int convert_yuv_dev(Workspace& ws, DevImage* img, int src_cg, int dst_cg, bool in_place = true);

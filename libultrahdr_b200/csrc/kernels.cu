@@ -505,6 +505,12 @@ __device__ __forceinline__ void apply_one(const ApplyParams& p, int x, int y, C3
     h.r = h.r < 0.0f ? 0.0f : (h.r > kMax ? kMax : h.r);
     h.g = h.g < 0.0f ? 0.0f : (h.g > kMax ? kMax : h.g);
     h.b = h.b < 0.0f ? 0.0f : (h.b > kMax ? kMax : h.b);
+    // a NaN passes the clamp as in the reference (0 * inf or inf - inf once max_content_boost puts +inf
+    // into the gain table); the reference's is x86's default NaN 0xFFC00000, the device's 0x7FFFFFFF
+    const float kNaN = __uint_as_float(0xFFC00000u);
+    if (h.r != h.r) h.r = kNaN;
+    if (h.g != h.g) h.g = kNaN;
+    if (h.b != h.b) h.b = kNaN;
     out[0] = float_to_half_ref(h.r) | (float_to_half_ref(h.g) << 16);
     out[1] = float_to_half_ref(h.b) | (0x3C00u << 16);
   } else {

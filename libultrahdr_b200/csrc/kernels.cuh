@@ -76,6 +76,7 @@ struct ApplyParams {                // applyGainMap, jpegr.cpp:1533-1831
   const float* luts;
   void* dst;
   int dst_stride;
+  int nan_possible;                 // the gain table is so large that a channel can become inf or NaN
 };
 
 struct TonemapParams {              // toneMap, jpegr.cpp:1985-2222

@@ -37,6 +37,10 @@ __device__ const unsigned long long kExp2fTab[32] = {
 __device__ __forceinline__ float powf_glibc(float x, float y) {
   unsigned ix = __float_as_uint(x);
   if (ix == 0u) return 0.0f;  // pow(+0, y > 0)
+  // pow(NaN, y) = NaN, as e_powf.c's special-case branch returns.  Without this the NaN's bits would go
+  // through the log as a number near 2^129, and a table index taken from the result overflows.  A NaN
+  // reaches here from applyGainMap's HLG output when max_content_boost puts +inf into the gain table.
+  if (x != x) return x;
   if (ix < 0x00800000u) {     // subnormal x: normalise like e_powf.c
     ix = __float_as_uint(x * 0x1p23f);
     ix &= 0x7fffffffu;

@@ -14,6 +14,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <limits>
 #include <memory>
 #include <vector>
 
@@ -229,6 +230,23 @@ int main(int argc, char** argv) {
     st = lib.applyGainMap(&s, gmap.get(), &gmd, UHDR_CT_LINEAR, UHDR_IMG_FMT_64bppRGBAHalfFloat, FLT_MAX, &dst);
     CHECK(st.error_code == UHDR_CODEC_OK);
     printf("applyGainMap gamut %d %016llx\n", (int)dst.cg, (unsigned long long)fnv(dst.planes[0], (size_t)kW * kH * 8));
+    // metadata that uhdr_validate_gainmap_metadata_descriptor refuses: one case per rule, and non-finite fields
+    for (int k = 0; k < 9; k++) {
+      uhdr_gainmap_metadata_ext_t bad = gmd;
+      switch (k) {
+        case 0: bad.max_content_boost[1] = bad.min_content_boost[1] * 0.5f; break;
+        case 1: bad.min_content_boost[0] = 0.0f; break;
+        case 2: bad.gamma[2] = 0.0f; break;
+        case 3: bad.offset_sdr[1] = -1e-3f; break;
+        case 4: bad.offset_hdr[0] = -1e-7f; break;
+        case 5: bad.hdr_capacity_max = bad.hdr_capacity_min; break;
+        case 6: bad.hdr_capacity_min = 0.5f; break;
+        case 7: bad.max_content_boost[0] = std::numeric_limits<float>::quiet_NaN(); break;
+        default: bad.gamma[0] = std::numeric_limits<float>::infinity(); break;
+      }
+      st = lib.applyGainMap(&s, gmap.get(), &bad, UHDR_CT_LINEAR, UHDR_IMG_FMT_64bppRGBAHalfFloat, FLT_MAX, &dst);
+      printf("applyGainMap invalid metadata %d: error %d\n", k, (int)st.error_code);
+    }
     uhdr_raw_image_ext_t tm(UHDR_IMG_FMT_12bppYCbCr420, UHDR_CG_UNSPECIFIED, UHDR_CT_UNSPECIFIED, UHDR_CR_UNSPECIFIED, kW, kH, 1);
     st = lib.toneMap(&h, &tm);
     CHECK(st.error_code == UHDR_CODEC_OK);
