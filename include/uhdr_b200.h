@@ -86,6 +86,51 @@ UHDR_EXTERN int uhdr_b200_jpeg_forward(const uhdr_raw_image_t* img, int quality,
 UHDR_EXTERN int uhdr_b200_jpeg_decode(const void* data, size_t size, int mode, uhdr_raw_image_t* out,
                                       size_t cap);
 
+/* The whole-file codec on DEVICE images: decodeJPEGR into device planes, encodeJPEGR from device intents and
+ * compressImage of a device image.  The compressed bytes stay in HOST memory.  Contract of all three:
+ *  - Device images: every plane pointer of a descriptor is device memory of the current device (checked with
+ *    cudaPointerGetAttributes), aligned to its element only (a sample of the planar formats, a pixel of the packed
+ *    ones, a byte for RGB888).  Strides are in pixels and may be any value >= the plane width.  Bytes between a
+ *    row's width and its stride are never read into a result and never written.  Inputs are never modified.
+ *  - Stream order (`stream`: the caller's cudaStream_t, NULL = the legacy default stream): writes into dest_dev /
+ *    gainmap_dev happen after all work enqueued earlier on `stream`, and work enqueued on it after the call sees
+ *    them without a host synchronise.  Encode inputs are read after the earlier work on `stream`.
+ *  - Host blocking: uhdr_b200_decode_dev may return before its pixels are written and does not wait for the work
+ *    enqueued on `stream` before it: the JPEG decoding runs on the library's own streams, only the writes into the
+ *    caller's planes are ordered onto `stream` (events).  A following call of any of the three on the same host
+ *    thread first waits on the host until those writes (or the kernels a failed decode left running) are done,
+ *    since they read the scratch memory it reuses: behind a busy stream, back-to-back decodes wait for the work
+ *    queued before the previous call.  The two encode calls run on `stream` and return when the file is complete.
+ *  - Errors: the codes of the host counterparts on the same input (uhdr_decode; uhdr_enc_set_raw_image plus
+ *    uhdr_encode; uhdr_b200_jpeg_encode).  Bad or host pointers, another device's memory, misalignment and wrong
+ *    dimensions give UHDR_CODEC_INVALID_PARAM.  A failing call writes nothing into the caller's device buffers.
+ *    Without a device: UHDR_CODEC_ERROR with a CUDA message.
+ *  - Threads: host threads with their own streams may call concurrently.  State is per host thread and device.
+ *
+ * uhdr_b200_decode_dev: JpegR::decodeJPEGR (ref lib/src/jpegr.cpp:1469-1531).  data/size: the JPEG/R file.
+ * dest_dev: fmt, w, h, stride[0] set by the caller, planes[0] a device pointer.  fmt and out_ct pair exactly as in
+ * uhdr_decode: RGBAHalfFloat + LINEAR, RGBA1010102 + HLG | PQ, RGBA8888 + SRGB (base image only).  w / h equal the
+ * primary image's (uhdr_dec_probe gives them).  On return dest_dev->cg / ct / range are filled in.
+ * gainmap_dev: optional.  w / h equal the map's, stride[0] >= w, the buffer holds h * stride[0] * 4 bytes.  The call
+ * sets fmt to Y400 or RGBA8888 and writes the decoded map (what uhdr_get_decoded_gainmap_image returns).
+ * metadata_out: optional host struct. */
+UHDR_EXTERN int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, float max_display_boost,
+                                     uhdr_raw_image_t* dest_dev, uhdr_raw_image_t* gainmap_dev,
+                                     uhdr_gainmap_metadata_t* metadata_out, void* stream);
+/* JpegR::encodeJPEGR API-1 (sdr_dev != NULL, ref lib/src/jpegr.cpp:247-291) / API-0 (sdr_dev == NULL, :179-244)
+ * from intents in device memory.  The JPEG/R file is written to the HOST buffer out (cap bytes); *out_size
+ * receives its length.  The bytes equal uhdr_encode's for the same intents and settings: cfg carries the settings
+ * uhdr_encode has (checked with its setters' ranges; FLT_MIN / FLT_MAX / -1 mean unset), and sdr_is_601 /
+ * use_luminance are ignored (uhdr_encode's values, 0 / 1, are used). */
+UHDR_EXTERN int uhdr_b200_encode_dev(const uhdr_raw_image_t* hdr_dev, const uhdr_raw_image_t* sdr_dev,
+                                     const uhdr_b200_gm_config_t* cfg, int base_quality,
+                                     const void* exif, size_t exif_size,
+                                     void* out, size_t cap, size_t* out_size, void* stream);
+/* JpegEncoderHelper::compressImage (ref lib/src/jpegencoderhelper.cpp:101) of a DEVICE image: the formats and
+ * bytes of uhdr_b200_jpeg_encode; the stream goes to the HOST buffer out. */
+UHDR_EXTERN int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img_dev, int quality, const void* icc,
+                                          size_t icc_size, void* out, size_t cap, size_t* out_size, void* stream);
+
 /* Measurement hooks.  Kernel timing brackets every kernel launch with CUDA events on the
  * launching stream and accumulates per-kernel totals ("name count total_ms min_ms max_ms" lines).
  * uhdr_b200_enc_rearm() makes a finished encoder handle runnable again while keeping the inputs

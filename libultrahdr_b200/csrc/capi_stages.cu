@@ -1,9 +1,12 @@
 // extern "C" stage entry points with HOST buffers (include/uhdr_b200.h): upload, run the device
 // stage, download, synchronise.  These are what the parity tests call through ctypes.
+#include <cmath>
 #include <cstring>
+#include <memory>
 #include <mutex>
+#include <vector>
 
-#include "engine.h"
+#include "codec.h"
 
 using namespace uhdr_b200;
 
@@ -306,6 +309,173 @@ UHDR_API int uhdr_b200_convert_yuv_dev(uhdr_raw_image_t* image, int src_cg, int 
   StreamScope scope(ws, stream);
   DevImage d = dev_view(*image);
   return convert_yuv_dev(*ws, &d, src_cg, dst_cg, /*in_place=*/true);
+}
+
+// ---- whole-file codec on device images -------------------------------------------------------------------
+namespace {
+// One codec per host thread and device (a handle is bound to the device that was current when it was made): a
+// decode needs its second workspace and parked helper thread.  settle() first: an earlier decode's writes into a
+// caller's planes may still read this codec's scratch.
+int dev_codec(JpegRCodec** out) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  static thread_local std::vector<std::unique_ptr<JpegRCodec>> per_device;
+  if ((int)per_device.size() <= dev) per_device.resize(dev + 1);
+  std::unique_ptr<JpegRCodec>& c = per_device[dev];
+  if (!c) {
+    c.reset(new JpegRCodec());
+    if (int rc = c->init()) {
+      c.reset();
+      return rc;
+    }
+  }
+  if (int rc = c->settle()) return rc;
+  c->ws().rewind();
+  *out = c.get();
+  return E_OK;
+}
+
+// the descriptor's planes: present, stride >= plane width, device memory of the current device, aligned to their
+// element (a sample of the planar formats, a pixel of the packed ones; RGB888 is read byte by byte)
+int check_dev_planes(const uhdr_raw_image_t& img, const char* what) {
+  const int np = fmt_planes(img.fmt);
+  if (np == 0) return fail(E_INVALID_PARAM, "%s: unsupported image format %d", what, img.fmt);
+  for (int i = 0; i < np; i++) {
+    int pw, ph, esz;
+    fmt_plane_geom(img.fmt, img.w, img.h, i, &pw, &ph, &esz);
+    if (!img.planes[i]) return fail(E_INVALID_PARAM, "%s: plane %d is a null pointer", what, i);
+    if ((int)img.stride[i] < pw) return fail(E_INVALID_PARAM, "%s: plane %d stride %u < width %d", what, i, img.stride[i], pw);
+    const int align = img.fmt == UHDR_IMG_FMT_24bppRGB888 ? 1 : esz;
+    if ((uintptr_t)img.planes[i] % align)
+      return fail(E_INVALID_PARAM, "%s: plane %d at %p is not aligned to its %d-byte elements", what, i, img.planes[i], align);
+  }
+  return E_OK;
+}
+int check_dev_memory(const uhdr_raw_image_t& img, const char* what) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  for (int i = 0; i < fmt_planes(img.fmt); i++) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, img.planes[i]) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(E_INVALID_PARAM, "%s: plane %d at %p is not a CUDA pointer", what, i, img.planes[i]);
+    }
+    if (a.type != cudaMemoryTypeDevice || a.device != dev)
+      return fail(E_INVALID_PARAM, "%s: plane %d at %p is not device memory of device %d", what, i, img.planes[i], dev);
+  }
+  return E_OK;
+}
+int check_out(const void* out, size_t* out_size) {
+  if (!out || !out_size) return fail(E_INVALID_PARAM, "received nullptr for the output buffer");
+  return E_OK;
+}
+}  // namespace
+
+UHDR_API int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
+                                  uhdr_raw_image_t* gainmap, uhdr_gainmap_metadata_t* metadata_out, void* stream) {
+  // uhdr_dec_set_image, uhdr_dec_set_out_max_display_boost and uhdr_decode's checks, in their order
+  if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed img->data field");
+  if (!dest) return fail(E_INVALID_PARAM, "received nullptr for destination image");
+  if (!std::isfinite(max_display_boost) || max_display_boost < 1.0f)
+    return fail(E_INVALID_PARAM, "invalid display boost %f, expects to be >= 1.0f}", max_display_boost);
+  DecodedInfo info;
+  int rc = JpegRCodec().probe((const uint8_t*)data, size, &info);  // host only
+  if (rc) return rc;
+  const int fmt = dest->fmt;
+  if ((fmt == UHDR_IMG_FMT_32bppRGBA1010102 && out_ct != UHDR_CT_HLG && out_ct != UHDR_CT_PQ) ||
+      (fmt == UHDR_IMG_FMT_64bppRGBAHalfFloat && out_ct != UHDR_CT_LINEAR) ||
+      (fmt == UHDR_IMG_FMT_32bppRGBA8888 && out_ct != UHDR_CT_SRGB) ||
+      (fmt != UHDR_IMG_FMT_32bppRGBA1010102 && fmt != UHDR_IMG_FMT_64bppRGBAHalfFloat && fmt != UHDR_IMG_FMT_32bppRGBA8888))
+    return fail(E_INVALID_PARAM, "unsupported output pixel format and output color transfer pair");
+  if ((int)dest->w != info.width || (int)dest->h != info.height)
+    return fail(E_INVALID_PARAM, "destination image is %ux%u, the primary image %dx%d", dest->w, dest->h, info.width, info.height);
+  if ((rc = check_dev_planes(*dest, "destination"))) return rc;
+  if (gainmap) {
+    if ((int)gainmap->w != info.gm_width || (int)gainmap->h != info.gm_height)
+      return fail(E_INVALID_PARAM, "gain-map image is %ux%u, the gain map %dx%d", gainmap->w, gainmap->h, info.gm_width,
+                  info.gm_height);
+    if (!gainmap->planes[0] || gainmap->stride[0] < gainmap->w)
+      return fail(E_INVALID_PARAM, "gain-map image: null plane or stride %u < width %u", gainmap->stride[0], gainmap->w);
+  }
+  JpegRCodec* c = nullptr;
+  if ((rc = dev_codec(&c))) return rc;
+  if ((rc = check_dev_memory(*dest, "destination"))) return rc;
+  if (gainmap) {
+    uhdr_raw_image_t g = *gainmap;
+    g.fmt = info.gm_channels == 1 ? UHDR_IMG_FMT_8bppYCbCr400 : UHDR_IMG_FMT_32bppRGBA8888;  // what the call writes
+    if ((rc = check_dev_planes(g, "gain-map image")) || (rc = check_dev_memory(g, "gain-map image"))) return rc;
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  return c->decode((const uint8_t*)data, size, out_ct, fmt, max_display_boost, dest, gainmap, metadata_out, &info, &st);
+}
+
+UHDR_API int uhdr_b200_encode_dev(const uhdr_raw_image_t* hdr, const uhdr_raw_image_t* sdr, const uhdr_b200_gm_config_t* cfg,
+                                  int base_quality, const void* exif, size_t exif_size, void* out, size_t cap,
+                                  size_t* out_size, void* stream) {
+  // uhdr_enc_set_raw_image per intent, the setters' ranges for the configuration, then uhdr_encode
+  if (!hdr) return fail(E_INVALID_PARAM, "received nullptr for raw image handle");
+  int rc = validate_raw_intent(*hdr, UHDR_HDR_IMG);
+  if (rc) return rc;
+  if (sdr) {
+    if ((rc = validate_raw_intent(*sdr, UHDR_SDR_IMG))) return rc;
+    if (sdr->w != hdr->w || sdr->h != hdr->h)
+      return fail(E_INVALID_PARAM, "image resolutions mismatch: hdr intent: %dx%d, sdr intent: %dx%d", hdr->w, hdr->h, sdr->w, sdr->h);
+  }
+  if (!cfg) return fail(E_INVALID_PARAM, "received nullptr for the gain-map configuration");
+  // the setters' ranges (uhdr_enc_set_quality, _gainmap_scale_factor, _gainmap_gamma, _preset,
+  // _min_max_content_boost, _target_display_peak_brightness); FLT_MIN / FLT_MAX / -1 = unset pass as they do there
+  if (base_quality < 0 || base_quality > 100 || cfg->quality < 0 || cfg->quality > 100)
+    return fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", base_quality, cfg->quality);
+  if (cfg->scale_factor <= 0 || cfg->scale_factor > 128)
+    return fail(E_INVALID_PARAM, "gainmap scale factor is expected to be in range (0, 128], received %d", cfg->scale_factor);
+  if (!std::isfinite(cfg->gamma) || cfg->gamma <= 0.0f)
+    return fail(E_INVALID_PARAM, "unsupported gainmap gamma %f, expects to be > 0", cfg->gamma);
+  if (cfg->preset != UHDR_USAGE_REALTIME && cfg->preset != UHDR_USAGE_BEST_QUALITY)
+    return fail(E_INVALID_PARAM, "invalid preset %d, expects one of {UHDR_USAGE_REALTIME, UHDR_USAGE_BEST_QUALITY}", cfg->preset);
+  const float mn = cfg->min_content_boost, mx = cfg->max_content_boost, nits = cfg->target_disp_peak_nits;
+  if (!std::isfinite(mn) || !std::isfinite(mx))
+    return fail(E_INVALID_PARAM, "received an argument with value either NaN or infinite. Configured min boost %f, max boost %f", mx, mn);
+  if (mx < mn)
+    return fail(E_INVALID_PARAM, "Invalid min boost / max boost configuration. configured max boost %f is less than min boost %f", mx, mn);
+  if (mn <= 0.0f) return fail(E_INVALID_PARAM, "Invalid min boost configuration %f, expects > 0.0f", mn);
+  if (nits != -1.0f && (!std::isfinite(nits) || nits < 203.0f || nits > 10000.0f))
+    return fail(E_INVALID_PARAM, "unexpected target display peak brightness nits %f, expects to be with in range [%f, %f]", nits,
+                203.0f, 10000.0f);
+  if (exif_size && !exif) return fail(E_INVALID_PARAM, "received nullptr for exif->data field");
+  if ((rc = check_out(out, out_size))) return rc;
+  if ((rc = check_dev_planes(*hdr, "hdr intent")) || (sdr && (rc = check_dev_planes(*sdr, "sdr intent")))) return rc;
+  JpegRCodec* c = nullptr;
+  if ((rc = dev_codec(&c))) return rc;
+  if ((rc = check_dev_memory(*hdr, "hdr intent")) || (sdr && (rc = check_dev_memory(*sdr, "sdr intent")))) return rc;
+  // on the caller's stream: the inputs are read after its earlier work; the call returns with the file complete
+  c->ws().use_external_stream((cudaStream_t)stream);
+  const DevImage dh = dev_view(*hdr), ds = sdr ? dev_view(*sdr) : DevImage{};
+  uhdr_b200_gm_config_t gcfg = *cfg;
+  gcfg.sdr_is_601 = 0;     // what uhdr_encode passes to generateGainMap
+  gcfg.use_luminance = 1;
+  rc = c->encode(dh, sdr ? &ds : nullptr, gcfg, base_quality, (const uint8_t*)exif, exif_size, (uint8_t*)out, cap, out_size,
+                 /*caller_planes=*/true);
+  if (rc) c->ws().sync();  // an error return can leave work in flight that reads the workspace
+  c->ws().clear_external_stream();
+  return rc;
+}
+
+UHDR_API int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img, int quality, const void* icc, size_t icc_size, void* out,
+                                       size_t cap, size_t* out_size, void* stream) {
+  if (!img) return fail(E_INVALID_PARAM, "received nullptr argument");
+  if (img->w == 0 || img->h == 0) return fail(E_INVALID_PARAM, "image has zero dimension");
+  int rc = check_out(out, out_size);
+  if (rc) return rc;
+  if ((rc = check_dev_planes(*img, "image"))) return rc;
+  JpegRCodec* c = nullptr;
+  if ((rc = dev_codec(&c))) return rc;
+  if ((rc = check_dev_memory(*img, "image"))) return rc;
+  c->ws().use_external_stream((cudaStream_t)stream);
+  rc = compress_image_dev(c->ws(), dev_view(*img), quality, icc, icc_size, /*caller_planes=*/true, (uint8_t*)out, cap,
+                          out_size);
+  if (rc) c->ws().sync();
+  c->ws().clear_external_stream();
+  return rc;
 }
 
 }  // extern "C"

@@ -23,9 +23,63 @@ static int block_stage(Workspace& ws, const DevImage& img, int quality, JpegEnco
   return jpeg_entropy_dev(ws, job);
 }
 
+// The block stage loads whole 8-sample rows of 8-byte aligned blocks (fdct8.cu).  A caller's device plane is
+// read as it is only when that touches nothing past the width: 8-byte aligned rows and a plane width that is a
+// multiple of 8 (RGB888 replicates its last column instead).  Otherwise it is staged into a workspace copy with
+// zero tails -- what upload_image makes of a host image, so the bytes equal those of the host entry points.
+static int block_stage_input(Workspace& ws, DevImage* img) {
+  bool direct = true;
+  for (int i = 0; i < fmt_planes(img->v.fmt); i++) {
+    int pw, ph, esz;
+    fmt_plane_geom(img->v.fmt, img->v.w, img->v.h, i, &pw, &ph, &esz);
+    direct = direct && (uintptr_t)img->v.p[i] % 8 == 0 && (size_t)img->v.stride[i] * esz % 8 == 0 &&
+             (img->v.fmt == F_RGB888 || pw % 8 == 0);
+  }
+  if (direct) return E_OK;
+  uhdr_raw_image_t src;
+  memset(&src, 0, sizeof src);
+  src.fmt = (uhdr_img_fmt_t)img->v.fmt;
+  src.w = img->v.w;
+  src.h = img->v.h;
+  src.cg = (uhdr_color_gamut_t)img->cg;
+  src.ct = (uhdr_color_transfer_t)img->ct;
+  src.range = (uhdr_color_range_t)img->range;
+  for (int i = 0; i < 3; i++) {
+    src.planes[i] = const_cast<void*>(img->v.p[i]);
+    src.stride[i] = img->v.stride[i];
+  }
+  return upload_image(ws, src, img, cudaMemcpyDeviceToDevice);
+}
+
+int compress_image_dev(Workspace& ws, const DevImage& img_in, int quality, const void* icc, size_t icc_size,
+                       bool caller_planes, uint8_t* out, size_t cap, size_t* out_size) {
+  DevImage img = img_in;
+  int rc = caller_planes ? block_stage_input(ws, &img) : E_OK;
+  if (rc) return rc;
+  JpegEncodeJob job;
+  rc = jpeg_forward_dev(ws, img, quality, &job, /*zigzag=*/true);
+  if (rc) return rc;
+  rc = jpeg_entropy_dev(ws, &job);
+  if (rc) return rc;
+  rc = ws.sync();
+  if (rc) return rc;
+  rc = jpeg_entropy_fetch(ws, &job);
+  if (rc) return rc;
+  rc = ws.sync();
+  if (rc) return rc;
+  std::vector<uint8_t> s;
+  const bool gm = img.v.fmt == F_RGB888 || img.v.fmt == F_Y400;  // the reference's is_gainmap_comment
+  rc = jpeg_finish_stream(job, icc, icc_size, gm ? jpeg_gainmap_comment() : nullptr, &s);
+  if (rc) return rc;
+  if (s.size() > cap) return fail(E_MEM, "output buffer too small: need %zu bytes", s.size());
+  memcpy(out, s.data(), s.size());
+  *out_size = s.size();
+  return E_OK;
+}
+
 int JpegRCodec::encode(const DevImage& hdr, const DevImage* sdr_in, const uhdr_b200_gm_config_t& cfg_in,
                        int base_quality, const uint8_t* exif, size_t exif_size, uint8_t* out, size_t cap,
-                       size_t* out_size) {
+                       size_t* out_size, bool caller_planes) {
   uhdr_b200_gm_config_t cfg = cfg_in;
   DevImage sdr;
   int rc;
@@ -65,6 +119,8 @@ int JpegRCodec::encode(const DevImage& hdr, const DevImage* sdr_in, const uhdr_b
     // can be encoded again): never convert it in place
     rc = convert_yuv_dev(ws_, &sdr, sdr.cg, UHDR_CG_DISPLAY_P3, /*in_place=*/false);
     if (rc) return rc;
+    // a Display-P3 intent is still the caller's plane
+    if (caller_planes && sdr.v.p[0] == sdr_in->v.p[0] && (rc = block_stage_input(ws_, &sdr))) return rc;
   }
   rc = block_stage(ws_, sdr, base_quality, &base_jpeg);
   if (rc) return rc;
@@ -295,9 +351,13 @@ void ParkedThread::wait() {
 
 JpegRCodec::~JpegRCodec() {
   if (map_ready_) cudaEventDestroy(map_ready_);
+  settle();
+  if (caller_ready_) cudaEventDestroy(caller_ready_);
+  if (writes_done_) cudaEventDestroy(writes_done_);
 }
 
-int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* h) {
+int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* h,
+                                YccToRgbaParams* to_rgba) {
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed image data");
   if (size == 0) return fail(E_INVALID_PARAM, "received bad compressed image size %zd", size);
   int rc = jpeg_read_header(data, size, h);
@@ -352,8 +412,12 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
         f.comp[1].v_samp != 1 || f.comp[2].h_samp != 1 || f.comp[2].v_samp != 1)
       return fail(E_UNSUPPORTED, "RGB output is implemented for 4:4:4, 4:2:2 and 4:2:0 JPEG input");
     DevImage rgba;
-    rc = alloc_dev_image(ws, F_RGBA8888, f.width, f.height, 1, &rgba);
-    if (rc) return rc;
+    if (to_rgba) {
+      out->v.fmt = F_RGBA8888;
+    } else {
+      rc = alloc_dev_image(ws, F_RGBA8888, f.width, f.height, 1, &rgba);
+      if (rc) return rc;
+    }
     YccToRgbaParams p;
     p.y = planes[0]; p.cb = planes[1]; p.cr = planes[2];
     p.src_stride = strides[0];
@@ -364,6 +428,10 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     p.c_stride = strides[1];
     p.cw = (f.width + f.max_h - 1) / f.max_h;
     p.ch = (f.height + f.max_v - 1) / f.max_v;
+    if (to_rgba) {
+      *to_rgba = p;
+      return E_OK;
+    }
     p.dst = (uint8_t*)rgba.v.p[0];
     p.dst_stride = rgba.v.stride[0];
     TIMED(ws, "ycc_to_rgba", launch_ycc_to_rgba(p, ws.stream()));
@@ -399,6 +467,7 @@ int JpegRCodec::probe(const uint8_t* data, size_t size, DecodedInfo* info) {
   info->height = ph.frame.height;
   info->gm_width = gh.frame.width;
   info->gm_height = gh.frame.height;
+  info->gm_channels = gh.frame.ncomp;
   info->base_off = po; info->base_len = pl;
   info->gainmap_off = go; info->gainmap_len = gl;
   info->exif = find_marker(data + po, ph, 0xE1, "Exif\0\0", 6);   // views into the caller's stream
@@ -413,12 +482,24 @@ int JpegRCodec::probe(const uint8_t* data, size_t size, DecodedInfo* info) {
 
 int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                        uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                       const DecodedInfo* probed) {
+                       const DecodedInfo* probed, const cudaStream_t* dev_stream) {
+  int rc = settle();
+  if (rc) return rc;
+  rc = decode_body(data, size, out_ct, out_fmt, max_display_boost, dest, gainmap_out, md_out, probed, dev_stream);
+  // an error can leave kernels of both JPEGs in flight on this codec's streams; the next call on it may run on a
+  // caller's stream that is not ordered against them, so settle() has to wait for them before the scratch is reused
+  if (rc) mark_in_flight();
+  return rc;
+}
+
+int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
+                            uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
+                            const DecodedInfo* probed, const cudaStream_t* dev_stream) {
   (void)out_fmt;
   PhaseTrace tr;
+  int rc = E_OK;
   ws_.rewind();
   size_t po, pl, go, gl;
-  int rc = E_OK;
   if (probed && probed->base_len && probed->gainmap_len && probed->gainmap_off + probed->gainmap_len <= size) {
     po = probed->base_off; pl = probed->base_len; go = probed->gainmap_off; gl = probed->gainmap_len;
   } else {
@@ -459,7 +540,10 @@ int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt
       else if (cudaEventRecord(j.self->map_ready_, j.self->ws2_->stream()) != cudaSuccess) fail_with(E_ERROR, "cudaEventRecord failed");
     }, &mj);
   }
-  rc = decode_jpeg_dev(ws_, data + po, pl, sdr_only ? 1 : 0, &sdr, &ph);  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS
+  // into device planes, the colour conversion of an SRGB output writes the caller's plane: it waits for the end
+  YccToRgbaParams to_rgba{};
+  rc = decode_jpeg_dev(ws_, data + po, pl, sdr_only ? 1 : 0, &sdr, &ph,
+                       dev_stream && sdr_only ? &to_rgba : nullptr);  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS
   if (overlap) helper_.wait();
   if (rc) return rc;
   tr.mark("primary jpeg enqueued");
@@ -490,6 +574,11 @@ int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt
     rc = parse_gainmap_metadata(blob.data, blob.size, xmp.data, xmp.size, exif.data, exif.size, &md);
     if (rc) return rc;
     if (md_out) *md_out = md;
+  }
+  if (dev_stream) {
+    rc = write_dev_outputs(sdr, map, to_rgba, md, out_ct, max_display_boost, dest, gainmap_out, *dev_stream);
+    tr.mark("writes enqueued");
+    return rc;
   }
   if (gainmap_out) {
     gainmap_out->fmt = (uhdr_img_fmt_t)map.v.fmt;
@@ -539,6 +628,78 @@ int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt
   rc = ws_.sync();
   tr.mark("pixels on the host");
   return rc;
+}
+
+int JpegRCodec::settle() {
+  if (!writes_pending_) return E_OK;
+  writes_pending_ = false;
+  CUDA_TRY(cudaEventSynchronize(writes_done_));
+  return E_OK;
+}
+
+int JpegRCodec::mark_in_flight() {
+  if (!writes_done_) CUDA_TRY(cudaEventCreateWithFlags(&writes_done_, cudaEventDisableTiming));
+  if (ws2_) {  // the helper's stream joins this one (map_ready_ is free: the helper has returned)
+    CUDA_TRY(cudaEventRecord(map_ready_, ws2_->stream()));
+    CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), map_ready_, 0));
+  }
+  CUDA_TRY(cudaEventRecord(writes_done_, ws_.stream()));
+  writes_pending_ = true;
+  return E_OK;
+}
+
+// decode() into device planes: every check first, then the writes -- straight into the caller's planes, no
+// full-frame copy -- behind the caller's stream
+int JpegRCodec::write_dev_outputs(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
+                                  const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
+                                  uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, cudaStream_t caller) {
+  const bool sdr_only = out_ct == UHDR_CT_SRGB;
+  if ((int)dest->w != sdr.v.w || (int)dest->h != sdr.v.h)
+    return fail(E_INVALID_PARAM, "destination image is %ux%u, the decoded image %dx%d", dest->w, dest->h, sdr.v.w, sdr.v.h);
+  if (sdr_only && dest->fmt != UHDR_IMG_FMT_32bppRGBA8888)
+    return fail(E_INVALID_PARAM, "unsupported output pixel format and output color transfer pair");
+  const int map_esz = map.v.fmt == F_Y400 ? 1 : 4;
+  if (gainmap_out && ((int)gainmap_out->w != map.v.w || (int)gainmap_out->h != map.v.h))
+    return fail(E_INVALID_PARAM, "gain-map image is %ux%u, the decoded gain map %dx%d", gainmap_out->w, gainmap_out->h,
+                map.v.w, map.v.h);
+  if (!caller_ready_) CUDA_TRY(cudaEventCreateWithFlags(&caller_ready_, cudaEventDisableTiming));
+  CUDA_TRY(cudaEventRecord(caller_ready_, caller));
+  CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), caller_ready_, 0));
+  if (sdr_only) {
+    YccToRgbaParams p = to_rgba;
+    p.dst = (uint8_t*)dest->planes[0];
+    p.dst_stride = dest->stride[0];
+    TIMED(ws_, "ycc_to_rgba", launch_ycc_to_rgba(p, ws_.stream()));
+    dest->cg = (uhdr_color_gamut_t)sdr.cg;
+    dest->ct = UHDR_CT_UNSPECIFIED;
+  } else {
+    DevImage dst;
+    memset(&dst, 0, sizeof dst);
+    dst.v.fmt = dest->fmt;
+    dst.v.w = sdr.v.w;
+    dst.v.h = sdr.v.h;
+    dst.v.p[0] = dest->planes[0];
+    dst.v.stride[0] = dest->stride[0];
+    dst.cg = dst.ct = dst.range = -1;
+    int rc = apply_gainmap_dev(ws_, sdr, map, md, out_ct, max_display_boost, &dst);
+    if (rc) return rc;
+    dest->cg = (uhdr_color_gamut_t)dst.cg;
+    dest->ct = (uhdr_color_transfer_t)out_ct;
+  }
+  dest->range = UHDR_CR_FULL_RANGE;
+  if (gainmap_out) {  // after the pixels: a failing apply leaves the map untouched too
+    gainmap_out->fmt = (uhdr_img_fmt_t)map.v.fmt;
+    gainmap_out->cg = UHDR_CG_UNSPECIFIED;
+    gainmap_out->ct = UHDR_CT_UNSPECIFIED;
+    gainmap_out->range = UHDR_CR_FULL_RANGE;
+    CUDA_TRY(cudaMemcpy2DAsync(gainmap_out->planes[0], (size_t)gainmap_out->stride[0] * map_esz, map.v.p[0],
+                               (size_t)map.v.stride[0] * map_esz, (size_t)map.v.w * map_esz, map.v.h,
+                               cudaMemcpyDeviceToDevice, ws_.stream()));
+  }
+  // this codec's stream waits for the caller's: settle() keeps the next call off the scratch read above
+  if (int rc = mark_in_flight()) return rc;
+  CUDA_TRY(cudaStreamWaitEvent(caller, writes_done_, 0));
+  return E_OK;
 }
 
 int JpegRCodec::fetch_gainmap(uhdr_raw_image_t* gainmap_out) {

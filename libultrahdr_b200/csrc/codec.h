@@ -15,7 +15,7 @@
 namespace uhdr_b200 {
 
 struct DecodedInfo {
-  int width = 0, height = 0, gm_width = 0, gm_height = 0;
+  int width = 0, height = 0, gm_width = 0, gm_height = 0, gm_channels = 0;
   ByteView exif, icc;   // views into the probed stream (the caller keeps it alive: the C API handle owns a copy)
   size_t base_off = 0, base_len = 0, gainmap_off = 0, gainmap_len = 0;  // the two JPEGs inside the probed stream
   uhdr_gainmap_metadata_t metadata{};
@@ -45,9 +45,11 @@ class JpegRCodec {
   Workspace& ws() { return ws_; }
 
   // JpegR::encodeJPEGR API-1 (jpegr.cpp:247-291) when sdr_dev != nullptr, API-0 (:179-244)
-  // otherwise.  Inputs are device images previously uploaded on ws().stream().
+  // otherwise.  Inputs are device images previously uploaded on ws().stream(), or with `caller_planes` a caller's
+  // device planes (any pitch, element alignment, undefined bytes past the width: see block_stage_input).
   int encode(const DevImage& hdr, const DevImage* sdr, const uhdr_b200_gm_config_t& cfg, int base_quality,
-             const uint8_t* exif, size_t exif_size, uint8_t* out, size_t cap, size_t* out_size);
+             const uint8_t* exif, size_t exif_size, uint8_t* out, size_t cap, size_t* out_size,
+             bool caller_planes = false);
   // JpegR::encodeJPEGR API-2 (jpegr.cpp:294-324, sdr != nullptr) / API-3 (:326-386, the compressed SDR is
   // decoded on the device and the map is computed with BT.601 luma): gain map from the intents, its JPEG,
   // appended to the caller's compressed SDR image.  `sdr_jpg_cg`: gamut of the compressed image when it
@@ -67,9 +69,17 @@ class JpegRCodec {
   // JpegR::decodeJPEGR (jpegr.cpp:1469-1531).  dest: host descriptor with planes allocated by the
   // caller (fmt/stride set); gainmap_out optional host descriptor (planes allocated, Y400/RGBA8888).
   // `probed`: the result of probe() on the same stream (saves the second scan of the container), or null.
+  // With `dev_stream`, dest->planes[0] and gainmap_out->planes[0] are device memory (w / h equal to the decoded
+  // images', checked before anything is written): the decoding runs on this codec's streams, the writes into the
+  // two planes are ordered after the work enqueued earlier on *dev_stream, and *dev_stream waits for them.  The
+  // call returns without waiting for either; settle() (run by the next decode()) waits for the writes.
   int decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
              uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-             const DecodedInfo* probed = nullptr);
+             const DecodedInfo* probed = nullptr, const cudaStream_t* dev_stream = nullptr);
+  // Host wait until what an earlier decode() left in flight is done -- its writes into device planes, or the kernels
+  // of a failed call: its scratch (device arenas of both workspaces, the pinned gain tables still waiting for their
+  // copy) may be reused after this.
+  int settle();
 
   // With gainmap_out->planes[0] == nullptr and lazy_gainmap set, decode() only fills the descriptor's
   // geometry and keeps the map in HBM; fetch_gainmap() copies it out when somebody asks for it
@@ -84,16 +94,39 @@ class JpegRCodec {
   ~JpegRCodec();
 
  private:
-  int decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr);
+  // `to_rgba` (mode 1 only): the colour conversion is not launched; its parameters, all but the destination,
+  // are returned there, out->v.p[0] stays null
+  int decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr,
+                      YccToRgbaParams* to_rgba = nullptr);
+  int decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
+                  uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
+                  const DecodedInfo* probed, const cudaStream_t* dev_stream);
+  // record where this codec's streams are (both joined into ws_); settle() waits for that point
+  int mark_in_flight();
+  int write_dev_outputs(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
+                        const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
+                        uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, cudaStream_t caller);
   Workspace ws_;
   // second stream + arenas: the gain-map JPEG of a decode is processed by a helper thread while the
   // calling thread handles the primary image (both entropy decoders alternate host and device phases)
   std::unique_ptr<Workspace> ws2_;
   ParkedThread helper_;
   cudaEvent_t map_ready_ = nullptr;
+  // decode() into device planes: the caller's stream up to the call, and this codec's writes into its planes
+  cudaEvent_t caller_ready_ = nullptr, writes_done_ = nullptr;
+  bool writes_pending_ = false;
   bool lazy_gainmap_ = false, map_pending_ = false;
   DevImage last_map_{};
 };
+
+// JpegEncoderHelper::compressImage (jpegencoderhelper.cpp:101) of a device image, on ws.stream(); returns once the
+// stream is in `out`.  `caller_planes`: see block_stage_input.
+int compress_image_dev(Workspace& ws, const DevImage& img, int quality, const void* icc, size_t icc_size,
+                       bool caller_planes, uint8_t* out, size_t cap, size_t* out_size);
+
+// uhdr_enc_set_raw_image's checks of one intent's descriptor (ultrahdr_api.cpp:842-1025): its code, the last error
+// set.  The planes are not dereferenced.
+int validate_raw_intent(const uhdr_raw_image_t& img, int intent);
 
 
 }  // namespace uhdr_b200

@@ -79,7 +79,7 @@ static cudaError_t copy_plane_async(void* dst, size_t dpitch, const void* src, s
   return cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, kind, s);
 }
 
-int upload_image(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out) {
+int upload_image(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out, cudaMemcpyKind kind) {
   if (src.w == 0 || src.h == 0) return fail(E_INVALID_PARAM, "image has zero dimension");
   int rc = alloc_dev_image(ws, src.fmt, src.w, src.h, 64, out);
   if (rc) return rc;
@@ -94,8 +94,7 @@ int upload_image(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out) {
     fmt_plane_geom(src.fmt, src.w, src.h, i, &pw, &ph, &esz);
     if ((int)src.stride[i] < pw) pw = src.stride[i];
     CUDA_TRY(copy_plane_async((void*)out->v.p[i], (size_t)out->v.stride[i] * esz, src.planes[i],
-                              (size_t)src.stride[i] * esz, (size_t)pw * esz, ph,
-                              cudaMemcpyHostToDevice, ws.stream()));
+                              (size_t)src.stride[i] * esz, (size_t)pw * esz, ph, kind, ws.stream()));
   }
   return E_OK;
 }

@@ -21,7 +21,10 @@ inline bool fmt_is_rgb_host(int f) { return f == F_RGBAF16 || f == F_RGBA8888 ||
 void fmt_plane_geom(int fmt, int w, int h, int i, int* pw, int* ph, int* esz);
 
 int alloc_dev_image(Workspace& ws, int fmt, int w, int h, int stride_align, DevImage* out);
-int upload_image(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out);
+// a copy of `src` in workspace memory: strides aligned to 64 pixels, the bytes past each row's width zero.
+// kind = cudaMemcpyDeviceToDevice stages a caller's device image the same way.
+int upload_image(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out,
+                 cudaMemcpyKind kind = cudaMemcpyHostToDevice);
 int download_image(Workspace& ws, const DevImage& src, uhdr_raw_image_t* dst);
 
 struct GainmapJob {      // state between enqueue and metadata finish

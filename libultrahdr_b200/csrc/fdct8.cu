@@ -392,7 +392,7 @@ static int fdct_device_books(const uint32_t** out) {
     jpeg_std_codebook(3, host + 256);
     uint32_t* d = nullptr;
     CUDA_TRY(cudaMalloc(&d, sizeof host));
-    CUDA_TRY(cudaMemcpy(d, host, sizeof host, cudaMemcpyHostToDevice));
+    if (int rc = copy_sync(d, host, sizeof host, cudaMemcpyHostToDevice)) return rc;
     per_dev[dev] = d;
   }
   *out = per_dev[dev];

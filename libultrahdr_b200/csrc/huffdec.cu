@@ -527,7 +527,9 @@ int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, con
     cudaGetDevice(&dev);
     std::lock_guard<std::mutex> lk(zig_mu);
     if (dev < 0 || dev >= 64 || !zig_done[dev]) {
-      CUDA_TRY(cudaMemcpyToSymbol(kZigzagDev, kZigzag, 64, 0, cudaMemcpyHostToDevice));
+      void* zig = nullptr;
+      CUDA_TRY(cudaGetSymbolAddress(&zig, kZigzagDev));
+      if (int rc = copy_sync(zig, kZigzag, 64, cudaMemcpyHostToDevice)) return rc;
       if (dev >= 0 && dev < 64) zig_done[dev] = true;
     }
   }

@@ -490,7 +490,7 @@ static int device_books(const uint32_t** out) {
   for (int t = 0; t < 4; t++) jpeg_std_codebook(t, host + 256 * t);
   uint32_t* d = nullptr;
   CUDA_TRY(cudaMalloc(&d, sizeof host));
-  CUDA_TRY(cudaMemcpy(d, host, sizeof host, cudaMemcpyHostToDevice));
+  if (int rc = copy_sync(d, host, sizeof host, cudaMemcpyHostToDevice)) return rc;
   cached = d;
   cached_dev = dev;
   *out = d;

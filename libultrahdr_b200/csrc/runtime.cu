@@ -25,6 +25,16 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+int copy_sync(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
+  cudaStream_t s = nullptr;
+  CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  cudaError_t e = cudaMemcpyAsync(dst, src, bytes, kind, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  cudaStreamDestroy(s);
+  CUDA_TRY(e);
+  return E_OK;
+}
+
 // ---- LUT residency ------------------------------------------------------------------------------
 static std::mutex g_lut_mu;
 static std::map<int, float*> g_luts;  // device ordinal -> device blob
@@ -55,11 +65,7 @@ const float* device_luts() {
   }
   std::vector<float> host(kLutTotalFloats);
   build_lut_blob(host.data());
-  e = cudaMemcpy(d, host.data(), sizeof(float) * kLutTotalFloats, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    fail(E_ERROR, "LUT upload failed: %s", cudaGetErrorString(e));
-    return nullptr;
-  }
+  if (copy_sync(d, host.data(), sizeof(float) * kLutTotalFloats, cudaMemcpyHostToDevice) != E_OK) return nullptr;
   return d;
 }
 
@@ -69,7 +75,9 @@ int install_luts_from_device(const void* dptr) {
   std::lock_guard<std::mutex> lk(g_lut_mu);
   float* d = lut_slot(dev);
   if (!d) return fail(E_MEM, "cudaMalloc of LUT blob failed");
+  // on the legacy stream, after the broadcast that filled dptr; landed before any kernel of ours reads it
   CUDA_TRY(cudaMemcpy(d, dptr, sizeof(float) * kLutTotalFloats, cudaMemcpyDeviceToDevice));
+  CUDA_TRY(cudaStreamSynchronize(cudaStreamLegacy));
   return E_OK;
 }
 

@@ -30,6 +30,11 @@ int fail(int code, const char* fmt, ...);
                                __FILE__, __LINE__, #expr);                                 \
   } while (0)
 
+// Copy that has landed when it returns, for tables uploaded once and then read by kernels on any stream.  A plain
+// cudaMemcpy from pageable memory (or device to device) may return before its DMA completes, and it is ordered
+// only against the legacy stream: kernels on the library's non-blocking streams could read the table before it.
+int copy_sync(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind);
+
 // Device-resident LUT blob for the current device (built on first use, or installed from a
 // broadcast).  Returns nullptr + sets last error when no CUDA device is usable.
 const float* device_luts();
