@@ -117,6 +117,31 @@ UHDR_EXTERN int uhdr_b200_jpeg_decode(const void* data, size_t size, int mode, u
 UHDR_EXTERN int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, float max_display_boost,
                                      uhdr_raw_image_t* dest_dev, uhdr_raw_image_t* gainmap_dev,
                                      uhdr_gainmap_metadata_t* metadata_out, void* stream);
+/* Reduced-size decoding: both JPEGs of the file at 1/k size, k in {1, 2, 4, 8}, the way libjpeg-turbo decodes with
+ * scale_num = 1, scale_denom = k -- a reduced inverse DCT per 8x8 block (4x4, 2x2 or 1x1 samples), not a decode
+ * followed by a downscale.  The primary image and the gain map each come out ceil(w / k) x ceil(h / k).  Chroma is
+ * scaled up by the IDCT, as libjpeg does: a 4:2:0 primary decodes to a 4:4:4 image at 1/k.  For HDR outputs the gain
+ * map is then applied as uhdr_decode applies it (applyGainMap on the two decoded images, with the file's metadata,
+ * out_ct and max_display_boost); an SRGB output is the primary image as RGBA8888.  k = 1 is the full-size decode.
+ * k > 1 supports gray, 4:4:4 and 4:2:0 JPEGs; another sampling (4:2:2, 4:4:0, 4:1:1) gives
+ * UHDR_CODEC_UNSUPPORTED_FEATURE, and a k outside {1, 2, 4, 8} UHDR_CODEC_INVALID_PARAM.
+ *
+ * uhdr_b200_scaled_dims: the sizes the caller allocates for a decode at 1/k -- primary *w x *h, gain map
+ * *gm_w x *gm_h.  Reads the container only; needs no device.
+ * uhdr_b200_decode_scaled_dev: uhdr_b200_decode_dev at 1/k, with exactly its contract (device planes of any pitch,
+ * stream order through events, the next call's host wait, nothing written on failure, the same error codes).
+ * dest_dev and gainmap_dev have the sizes uhdr_b200_scaled_dims returns.  A small result is copied to the host by the
+ * caller: there is no host-buffer form. */
+UHDR_EXTERN int uhdr_b200_scaled_dims(const void* data, size_t size, int k, unsigned* w, unsigned* h, unsigned* gm_w,
+                                      unsigned* gm_h);
+UHDR_EXTERN int uhdr_b200_decode_scaled_dev(const void* data, size_t size, int k, int out_ct, float max_display_boost,
+                                            uhdr_raw_image_t* dest_dev, uhdr_raw_image_t* gainmap_dev,
+                                            uhdr_gainmap_metadata_t* metadata_out, void* stream);
+/* uhdr_b200_jpeg_decode of one JPEG at 1/k (stage hook, host buffers).  k = 1 is uhdr_b200_jpeg_decode.  For k > 1,
+ * mode 0 gives Y400 or YUV444 planes of ceil(w / k) x ceil(h / k) samples, back to back at stride = width; mode 1
+ * gives RGBA8888 at that size. */
+UHDR_EXTERN int uhdr_b200_jpeg_decode_scaled(const void* data, size_t size, int mode, int k, uhdr_raw_image_t* out,
+                                             size_t cap);
 /* JpegR::encodeJPEGR API-1 (sdr_dev != NULL, ref lib/src/jpegr.cpp:247-291) / API-0 (sdr_dev == NULL, :179-244)
  * from intents in device memory.  The JPEG/R file is written to the HOST buffer out (cap bytes); *out_size
  * receives its length.  The bytes equal uhdr_encode's for the same intents and settings: cfg carries the settings

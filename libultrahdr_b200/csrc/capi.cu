@@ -623,12 +623,12 @@ UHDR_API int uhdr_b200_jpeg_encode(const uhdr_raw_image_t* img, int quality, con
   return compress_image_dev(c->ws(), d, quality, icc, icc_size, /*caller_planes=*/false, (uint8_t*)out, cap, out_size);
 }
 
-UHDR_API int uhdr_b200_jpeg_decode(const void* data, size_t size, int mode, uhdr_raw_image_t* out, size_t cap) {
+static int jpeg_decode_host(const void* data, size_t size, int mode, int k, uhdr_raw_image_t* out, size_t cap) {
   JpegRCodec* c = tls_codec();
   if (!c) return E_ERROR;
   DevImage d;
   JpegHeader h;
-  int rc = c->decode_jpeg_dev((const uint8_t*)data, size, mode, &d, &h);
+  int rc = c->decode_jpeg_dev((const uint8_t*)data, size, mode, &d, &h, k);
   if (rc) return rc;
   // host layout of JpegDecoderHelper::getDecompressedImage (:536-552)
   const JpegFrame& f = h.frame;
@@ -647,6 +647,17 @@ UHDR_API int uhdr_b200_jpeg_decode(const void* data, size_t size, int mode, uhdr
     out->planes[1] = out->planes[2] = nullptr;
     out->stride[1] = out->stride[2] = 0;
     rc = download_image(c->ws(), d, out);
+  } else if (k != 1) {  // reduced size: every plane out w x h (Y400 / YUV444), back to back at stride w
+    need = (size_t)d.v.w * d.v.h * f.ncomp;
+    if (need > cap) return fail(E_MEM, "output buffer too small: need %zu bytes", need);
+    uint8_t* p = base;
+    for (int i = 0; i < 3; i++) {
+      out->planes[i] = i < f.ncomp ? p : nullptr;
+      out->stride[i] = i < f.ncomp ? d.v.w : 0;
+      if (i < f.ncomp)
+        CUDA_TRY(cudaMemcpy2DAsync(p, d.v.w, d.v.p[i], d.v.stride[i], d.v.w, d.v.h, cudaMemcpyDeviceToHost, c->ws().stream()));
+      if (i < f.ncomp) p += (size_t)d.v.w * d.v.h;
+    }
   } else {
     unsigned hs[3] = {0, 0, 0}, vs[3] = {0, 0, 0};
     for (int k = 0; k < f.ncomp; k++) {
@@ -670,6 +681,16 @@ UHDR_API int uhdr_b200_jpeg_decode(const void* data, size_t size, int mode, uhdr
   }
   if (rc) return rc;
   return c->ws().sync();
+}
+
+UHDR_API int uhdr_b200_jpeg_decode(const void* data, size_t size, int mode, uhdr_raw_image_t* out, size_t cap) {
+  return jpeg_decode_host(data, size, mode, 1, out, cap);
+}
+
+UHDR_API int uhdr_b200_jpeg_decode_scaled(const void* data, size_t size, int mode, int k, uhdr_raw_image_t* out, size_t cap) {
+  if (k != 1 && k != 2 && k != 4 && k != 8) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
+  if (!data || !out || !out->planes[0]) return fail(E_INVALID_PARAM, "received nullptr argument");
+  return jpeg_decode_host(data, size, mode, k, out, cap);
 }
 
 UHDR_API int uhdr_b200_encode_batch(int n, const uhdr_raw_image_t* hdr, const uhdr_raw_image_t* sdr,

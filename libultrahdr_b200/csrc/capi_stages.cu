@@ -365,14 +365,23 @@ int check_dev_memory(const uhdr_raw_image_t& img, const char* what) {
   }
   return E_OK;
 }
+bool valid_scale(int k) { return k == 1 || k == 2 || k == 4 || k == 8; }
+// the probed sizes at 1/k: libjpeg's output size of a scale_denom = k decode, ceil(size / k)
+void scale_dims(DecodedInfo* info, int k) {
+  info->width = (info->width + k - 1) / k;
+  info->height = (info->height + k - 1) / k;
+  info->gm_width = (info->gm_width + k - 1) / k;
+  info->gm_height = (info->gm_height + k - 1) / k;
+}
 int check_out(const void* out, size_t* out_size) {
   if (!out || !out_size) return fail(E_INVALID_PARAM, "received nullptr for the output buffer");
   return E_OK;
 }
 }  // namespace
 
-UHDR_API int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
-                                  uhdr_raw_image_t* gainmap, uhdr_gainmap_metadata_t* metadata_out, void* stream) {
+// uhdr_b200_decode_dev (k = 1) and uhdr_b200_decode_scaled_dev: sizes checked against the 1/k ones
+static int decode_dev(const void* data, size_t size, int k, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
+                      uhdr_raw_image_t* gainmap, uhdr_gainmap_metadata_t* metadata_out, void* stream) {
   // uhdr_dec_set_image, uhdr_dec_set_out_max_display_boost and uhdr_decode's checks, in their order
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed img->data field");
   if (!dest) return fail(E_INVALID_PARAM, "received nullptr for destination image");
@@ -381,6 +390,7 @@ UHDR_API int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, flo
   DecodedInfo info;
   int rc = JpegRCodec().probe((const uint8_t*)data, size, &info);  // host only
   if (rc) return rc;
+  scale_dims(&info, k);
   const int fmt = dest->fmt;
   if ((fmt == UHDR_IMG_FMT_32bppRGBA1010102 && out_ct != UHDR_CT_HLG && out_ct != UHDR_CT_PQ) ||
       (fmt == UHDR_IMG_FMT_64bppRGBAHalfFloat && out_ct != UHDR_CT_LINEAR) ||
@@ -406,7 +416,34 @@ UHDR_API int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, flo
     if ((rc = check_dev_planes(g, "gain-map image")) || (rc = check_dev_memory(g, "gain-map image"))) return rc;
   }
   const cudaStream_t st = (cudaStream_t)stream;
-  return c->decode((const uint8_t*)data, size, out_ct, fmt, max_display_boost, dest, gainmap, metadata_out, &info, &st);
+  return c->decode((const uint8_t*)data, size, out_ct, fmt, max_display_boost, dest, gainmap, metadata_out, &info, &st, k);
+}
+
+UHDR_API int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
+                                  uhdr_raw_image_t* gainmap, uhdr_gainmap_metadata_t* metadata_out, void* stream) {
+  return decode_dev(data, size, 1, out_ct, max_display_boost, dest, gainmap, metadata_out, stream);
+}
+
+UHDR_API int uhdr_b200_decode_scaled_dev(const void* data, size_t size, int k, int out_ct, float max_display_boost,
+                                         uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap,
+                                         uhdr_gainmap_metadata_t* metadata_out, void* stream) {
+  if (!valid_scale(k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
+  return decode_dev(data, size, k, out_ct, max_display_boost, dest, gainmap, metadata_out, stream);
+}
+
+UHDR_API int uhdr_b200_scaled_dims(const void* data, size_t size, int k, unsigned* w, unsigned* h, unsigned* gm_w,
+                                   unsigned* gm_h) {
+  if (!valid_scale(k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
+  if (!data || !w || !h || !gm_w || !gm_h) return fail(E_INVALID_PARAM, "received nullptr argument");
+  DecodedInfo info;
+  int rc = JpegRCodec().probe((const uint8_t*)data, size, &info);  // host only, no device needed
+  if (rc) return rc;
+  scale_dims(&info, k);
+  *w = info.width;
+  *h = info.height;
+  *gm_w = info.gm_width;
+  *gm_h = info.gm_height;
+  return E_OK;
 }
 
 UHDR_API int uhdr_b200_encode_dev(const uhdr_raw_image_t* hdr, const uhdr_raw_image_t* sdr, const uhdr_b200_gm_config_t* cfg,

@@ -1,5 +1,6 @@
 #include "codec.h"
 
+#include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -357,7 +358,7 @@ JpegRCodec::~JpegRCodec() {
 }
 
 int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* h,
-                                YccToRgbaParams* to_rgba) {
+                                YccToRgbaParams* to_rgba, int k) {
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed image data");
   if (size == 0) return fail(E_INVALID_PARAM, "received bad compressed image size %zd", size);
   int rc = jpeg_read_header(data, size, h);
@@ -369,17 +370,29 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
   if (h->adobe_transform == 0 && f.ncomp == 3)
     return fail(E_UNSUPPORTED, "RGB (Adobe transform 0) JPEG input is not supported by the CUDA decoder");
   if (mode == 1 && f.ncomp == 1) return fail(E_ERROR, "expected input color space to be JCS_YCbCr or JCS_RGB but got %d", 1);
+  // reduced size (k > 1): every component must come out of the IDCT at the output size; other samplings would
+  // need libjpeg's upsampler at the reduced size
+  const bool scaled = k != 1;
+  JpegScaled g;
+  if (scaled) {
+    if ((rc = jpeg_scaled_geometry(f, k, &g))) return rc;
+    if (!g.full_chroma())
+      return fail(E_UNSUPPORTED, "decoding at 1/%d size is implemented for gray, 4:4:4 and 4:2:0 JPEG input", k);
+  }
   memset(out, 0, sizeof *out);
   out->cg = out->ct = -1;
   out->range = UHDR_CR_FULL_RANGE;
   out->v.full_range = 1;
-  out->v.w = f.width;
-  out->v.h = f.height;
+  out->v.w = scaled ? g.width : f.width;
+  out->v.h = scaled ? g.height : f.height;
   uint8_t* planes[3] = {nullptr, nullptr, nullptr};
   int strides[3] = {0, 0, 0};
+  // scaled planes share one stride: the 4:4:4 colour conversion and the apply kernels index chroma with luma's
+  int common = 0;
+  for (int c = 0; scaled && c < f.ncomp; c++) common = std::max(common, f.comp[c].wblocks * g.s[c]);
   for (int c = 0; c < f.ncomp; c++) {
-    strides[c] = f.comp[c].wblocks * 8;
-    planes[c] = (uint8_t*)ws.dalloc((size_t)strides[c] * f.comp[c].hblocks * 8);
+    strides[c] = scaled ? common : f.comp[c].wblocks * 8;
+    planes[c] = (uint8_t*)ws.dalloc((size_t)strides[c] * f.comp[c].hblocks * (scaled ? g.s[c] : 8));
     if (!planes[c]) return E_MEM;
   }
   // entropy decoding: on the device (huffdec.cu).  The host decoder is not a size-based alternative: it runs only
@@ -392,7 +405,7 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     rc = jpeg_entropy_decode_dev(ws, data, size, *h, d_coefs);
     if (rc == kHuffDecFallback) on_device = false;
     else if (rc) return rc;
-    else rc = jpeg_idct_dev(ws, *h, d_coefs, planes, strides);
+    else rc = scaled ? jpeg_idct_scaled_dev(ws, *h, g, d_coefs, planes, strides) : jpeg_idct_dev(ws, *h, d_coefs, planes, strides);
     if (on_device && rc) return rc;
   }
   if (!on_device) {
@@ -403,31 +416,31 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     }
     rc = jpeg_host_decode_coefs(data, size, *h, h_coefs);
     if (rc) return rc;
-    rc = jpeg_inverse_dev(ws, *h, h_coefs, planes, strides);
+    rc = scaled ? jpeg_inverse_scaled_dev(ws, *h, g, h_coefs, planes, strides) : jpeg_inverse_dev(ws, *h, h_coefs, planes, strides);
     if (rc) return rc;
   }
   if (mode == 1) {
     const bool s444 = f.max_h == 1 && f.max_v == 1, s422 = f.max_h == 2 && f.max_v == 1, s420 = f.max_h == 2 && f.max_v == 2;
-    if (!(s444 || s422 || s420) || f.comp[0].h_samp != f.max_h || f.comp[0].v_samp != f.max_v || f.comp[1].h_samp != 1 ||
-        f.comp[1].v_samp != 1 || f.comp[2].h_samp != 1 || f.comp[2].v_samp != 1)
+    if (!scaled && (!(s444 || s422 || s420) || f.comp[0].h_samp != f.max_h || f.comp[0].v_samp != f.max_v || f.comp[1].h_samp != 1 ||
+        f.comp[1].v_samp != 1 || f.comp[2].h_samp != 1 || f.comp[2].v_samp != 1))
       return fail(E_UNSUPPORTED, "RGB output is implemented for 4:4:4, 4:2:2 and 4:2:0 JPEG input");
     DevImage rgba;
     if (to_rgba) {
       out->v.fmt = F_RGBA8888;
     } else {
-      rc = alloc_dev_image(ws, F_RGBA8888, f.width, f.height, 1, &rgba);
+      rc = alloc_dev_image(ws, F_RGBA8888, out->v.w, out->v.h, 1, &rgba);
       if (rc) return rc;
     }
     YccToRgbaParams p;
     p.y = planes[0]; p.cb = planes[1]; p.cr = planes[2];
     p.src_stride = strides[0];
-    p.w = f.width;
-    p.h = f.height;
-    p.hs = f.max_h;
-    p.vs = f.max_v;
+    p.w = out->v.w;
+    p.h = out->v.h;
+    p.hs = scaled ? 1 : f.max_h;  // scaled: chroma at full resolution already (4:4:4)
+    p.vs = scaled ? 1 : f.max_v;
     p.c_stride = strides[1];
-    p.cw = (f.width + f.max_h - 1) / f.max_h;
-    p.ch = (f.height + f.max_v - 1) / f.max_v;
+    p.cw = (p.w + p.hs - 1) / p.hs;
+    p.ch = (p.h + p.vs - 1) / p.vs;
     if (to_rgba) {
       *to_rgba = p;
       return E_OK;
@@ -440,7 +453,7 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     out->cg = out->ct = -1;
     return E_OK;
   }
-  const int fmt = sampling_format(f);
+  const int fmt = scaled ? (f.ncomp == 1 ? F_Y400 : F_YUV444) : sampling_format(f);
   if (fmt < 0) return fail(E_ERROR, "unrecognized subsampling format for output color space JCS_YCbCr");
   out->v.fmt = fmt;
   for (int c = 0; c < f.ncomp; c++) {
@@ -482,10 +495,10 @@ int JpegRCodec::probe(const uint8_t* data, size_t size, DecodedInfo* info) {
 
 int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                        uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                       const DecodedInfo* probed, const cudaStream_t* dev_stream) {
+                       const DecodedInfo* probed, const cudaStream_t* dev_stream, int k) {
   int rc = settle();
   if (rc) return rc;
-  rc = decode_body(data, size, out_ct, out_fmt, max_display_boost, dest, gainmap_out, md_out, probed, dev_stream);
+  rc = decode_body(data, size, out_ct, out_fmt, max_display_boost, dest, gainmap_out, md_out, probed, dev_stream, k);
   // an error can leave kernels of both JPEGs in flight on this codec's streams; the next call on it may run on a
   // caller's stream that is not ordered against them, so settle() has to wait for them before the scratch is reused
   if (rc) mark_in_flight();
@@ -494,7 +507,7 @@ int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt
 
 int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                             uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                            const DecodedInfo* probed, const cudaStream_t* dev_stream) {
+                            const DecodedInfo* probed, const cudaStream_t* dev_stream, int k) {
   (void)out_fmt;
   PhaseTrace tr;
   int rc = E_OK;
@@ -519,9 +532,9 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
     size_t len;
     DevImage* map;
     JpegHeader* gh;
-    int dev, rc;
+    int dev, k, rc;
     char err[256];
-  } mj{this, data + go, gl, &map, &gh, 0, E_OK, {0}};
+  } mj{this, data + go, gl, &map, &gh, 0, k, E_OK, {0}};
   if (overlap) {
     if (!ws2_) {
       ws2_.reset(new Workspace());
@@ -535,7 +548,7 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
       MapJob& j = *static_cast<MapJob*>(a);
       auto fail_with = [&](int rc, const char* what) { j.rc = rc; snprintf(j.err, sizeof j.err, "%s", what); };
       if (cudaSetDevice(j.dev) != cudaSuccess) return fail_with(E_ERROR, "cudaSetDevice failed in the gain-map decode thread");
-      j.rc = j.self->decode_jpeg_dev(*j.self->ws2_, j.data, j.len, 2, j.map, j.gh);  // DECODE_STREAM :1486
+      j.rc = j.self->decode_jpeg_dev(*j.self->ws2_, j.data, j.len, 2, j.map, j.gh, nullptr, j.k);  // DECODE_STREAM :1486
       if (j.rc) snprintf(j.err, sizeof j.err, "%s", last_error());
       else if (cudaEventRecord(j.self->map_ready_, j.self->ws2_->stream()) != cudaSuccess) fail_with(E_ERROR, "cudaEventRecord failed");
     }, &mj);
@@ -543,7 +556,7 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
   // into device planes, the colour conversion of an SRGB output writes the caller's plane: it waits for the end
   YccToRgbaParams to_rgba{};
   rc = decode_jpeg_dev(ws_, data + po, pl, sdr_only ? 1 : 0, &sdr, &ph,
-                       dev_stream && sdr_only ? &to_rgba : nullptr);  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS
+                       dev_stream && sdr_only ? &to_rgba : nullptr, k);  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS
   if (overlap) helper_.wait();
   if (rc) return rc;
   tr.mark("primary jpeg enqueued");
@@ -557,7 +570,7 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
       CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), map_ready_, 0));
       if (kernel_timing_enabled()) ws2_->sync();
     } else {
-      rc = decode_jpeg_dev(ws_, data + go, gl, 2, &map, &gh);  // DECODE_STREAM :1486
+      rc = decode_jpeg_dev(ws_, data + go, gl, 2, &map, &gh, nullptr, k);  // DECODE_STREAM :1486
       if (rc) return rc;
     }
     blob = find_marker(data + go, gh, 0xE2, "ICC_PROFILE", 12);

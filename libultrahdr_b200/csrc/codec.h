@@ -73,9 +73,10 @@ class JpegRCodec {
   // images', checked before anything is written): the decoding runs on this codec's streams, the writes into the
   // two planes are ordered after the work enqueued earlier on *dev_stream, and *dev_stream waits for them.  The
   // call returns without waiting for either; settle() (run by the next decode()) waits for the writes.
+  // `k` (1, 2, 4, 8): both JPEGs are decoded at 1/k size (jpeg_scaled_geometry) and the gain map is applied to those.
   int decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
              uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-             const DecodedInfo* probed = nullptr, const cudaStream_t* dev_stream = nullptr);
+             const DecodedInfo* probed = nullptr, const cudaStream_t* dev_stream = nullptr, int k = 1);
   // Host wait until what an earlier decode() left in flight is done -- its writes into device planes, or the kernels
   // of a failed call: its scratch (device arenas of both workspaces, the pinned gain tables still waiting for their
   // copy) may be reused after this.
@@ -88,8 +89,9 @@ class JpegRCodec {
   int fetch_gainmap(uhdr_raw_image_t* gainmap_out);
 
   // JpegDecoderHelper::decompressImage equivalent producing a device image
-  int decode_jpeg_dev(const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr) {
-    return decode_jpeg_dev(ws_, data, size, mode, out, hdr);
+  // `k` > 1: at 1/k size, gray / 4:4:4 / 4:2:0 input only, the planes come out Y400 or YUV444 (jpeg_scaled_geometry)
+  int decode_jpeg_dev(const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr, int k = 1) {
+    return decode_jpeg_dev(ws_, data, size, mode, out, hdr, nullptr, k);
   }
   ~JpegRCodec();
 
@@ -97,10 +99,10 @@ class JpegRCodec {
   // `to_rgba` (mode 1 only): the colour conversion is not launched; its parameters, all but the destination,
   // are returned there, out->v.p[0] stays null
   int decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr,
-                      YccToRgbaParams* to_rgba = nullptr);
+                      YccToRgbaParams* to_rgba = nullptr, int k = 1);
   int decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                   uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                  const DecodedInfo* probed, const cudaStream_t* dev_stream);
+                  const DecodedInfo* probed, const cudaStream_t* dev_stream, int k);
   // record where this codec's streams are (both joined into ws_); settle() waits for that point
   int mark_in_flight();
   int write_dev_outputs(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,

@@ -108,6 +108,24 @@ int jpeg_inverse_dev(Workspace& ws, const JpegHeader& h, int16_t* const h_coefs[
                      uint8_t* d_planes[3], int plane_stride[3]);
 // Same, coefficients already on the device.
 int jpeg_idct_dev(Workspace& ws, const JpegHeader& h, int16_t* const d_coefs[3], uint8_t* d_planes[3], int plane_stride[3]);
+// Reduced-size decoding, libjpeg's scale_num = 1, scale_denom = k (jdmaster.c): the output is ceil(W/k) x ceil(H/k).
+// Every component starts at a DCT scaled size of 8/k samples per block side, doubled while that is < 8 and the
+// sampling factors allow it (chroma is scaled up by the IDCT, not by an upsampler): a 4:2:0 frame comes out 4:4:4.
+// Component c is w[c] x h[c] = ceil(W*h_samp*s / (max_h*8)) x ceil(H*v_samp*s / (max_v*8)).
+struct JpegScaled {
+  int k = 1, width = 0, height = 0;
+  int s[3] = {8, 8, 8}, w[3] = {0, 0, 0}, h[3] = {0, 0, 0};
+  bool full_chroma() const;  // every component at the output size (gray, 4:4:4, 4:2:0 at k > 1)
+};
+// E_INVALID_PARAM for k outside {1, 2, 4, 8}
+int jpeg_scaled_geometry(const JpegFrame& f, int k, JpegScaled* g);
+// Dequant + IDCT at the scaled sizes: components of size 8 through k_idct_dequant, the others through the reduced
+// IDCT (one launch per size).  Plane c holds hblocks*s[c] rows of wblocks*s[c] samples at plane_stride[c].
+int jpeg_idct_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const d_coefs[3],
+                         uint8_t* d_planes[3], int plane_stride[3]);
+// Same, coefficients decoded on the host.
+int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const h_coefs[3],
+                            uint8_t* d_planes[3], int plane_stride[3]);
 // Entropy decoding on the device (huffdec.cu): fills d_coefs[c] (allocated from the workspace) with
 // [block][64] natural-order coefficients.  Returns kHuffDecFallback when the stream is outside what
 // the parallel decoder handles (restart markers, no fixed point, inconsistent data): the caller then

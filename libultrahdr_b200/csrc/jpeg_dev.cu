@@ -107,6 +107,59 @@ int jpeg_inverse_dev(Workspace& ws, const JpegHeader& h, int16_t* const h_coefs[
   return jpeg_idct_dev(ws, h, d_coefs, d_planes, plane_stride);
 }
 
+int jpeg_idct_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const d_coefs[3],
+                         uint8_t* d_planes[3], int plane_stride[3]) {
+  const JpegFrame& f = h.frame;
+  for (int c = 0; c < f.ncomp; c++) {
+    if (g.s[c] != 8) continue;
+    const JpegComp& k = f.comp[c];
+    IdctPlaneParams p;
+    memset(&p, 0, sizeof p);
+    p.coefs = d_coefs[c];
+    memcpy(p.q, f.qt[k.tq], sizeof p.q);
+    p.wblocks = k.wblocks;
+    p.hblocks = k.hblocks;
+    p.dst = d_planes[c];
+    p.dst_stride = plane_stride[c];
+    p.dst_w = k.wblocks * 8 < plane_stride[c] ? k.wblocks * 8 : plane_stride[c];
+    p.dst_h = k.hblocks * 8;
+    TIMED(ws, "idct_dequant", launch_idct_dequant(p, ws.stream()));
+  }
+  for (int size = 4; size >= 1; size /= 2) {
+    IdctScaledParams p;
+    memset(&p, 0, sizeof p);
+    int blocks = 0;
+    for (int c = 0; c < f.ncomp; c++) {
+      if (g.s[c] != size) continue;
+      const JpegComp& k = f.comp[c];
+      IdctScaledParams::Plane& pl = p.plane[p.nplanes];
+      pl.coefs = d_coefs[c];
+      memcpy(pl.q, f.qt[k.tq], sizeof pl.q);
+      pl.wblocks = k.wblocks;
+      pl.dst = d_planes[c];
+      pl.dst_stride = plane_stride[c];
+      pl.dst_w = k.wblocks * size;
+      pl.dst_h = k.hblocks * size;
+      blocks += k.wblocks * k.hblocks;
+      p.block_end[p.nplanes++] = blocks;
+    }
+    if (p.nplanes) TIMED(ws, "idct_scaled", launch_idct_scaled(p, size, ws.stream()));
+  }
+  return E_OK;
+}
+
+int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const h_coefs[3],
+                            uint8_t* d_planes[3], int plane_stride[3]) {
+  const JpegFrame& f = h.frame;
+  int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
+  for (int c = 0; c < f.ncomp; c++) {
+    d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
+    if (!d_coefs[c]) return E_MEM;
+    CUDA_TRY(cudaMemcpyAsync(d_coefs[c], h_coefs[c], f.blocks(c) * 128, cudaMemcpyHostToDevice, ws.stream()));
+  }
+  return jpeg_idct_scaled_dev(ws, h, g, d_coefs, d_planes, plane_stride);
+}
+
 namespace {
 std::atomic<int> g_entropy_decoder{0};
 }

@@ -481,4 +481,29 @@ int jpeg_host_decode_coefs(const uint8_t* data, size_t size, const JpegHeader& h
   return E_OK;
 }
 
+int jpeg_scaled_geometry(const JpegFrame& f, int k, JpegScaled* g) {
+  if (k != 1 && k != 2 && k != 4 && k != 8) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
+  *g = JpegScaled();
+  g->k = k;
+  g->width = (f.width + k - 1) / k;
+  g->height = (f.height + k - 1) / k;
+  const int m = 8 / k;
+  for (int c = 0; c < f.ncomp; c++) {
+    const JpegComp& p = f.comp[c];
+    int s = m;
+    while (s < 8 && (f.max_h * m) % (p.h_samp * s * 2) == 0 && (f.max_v * m) % (p.v_samp * s * 2) == 0) s *= 2;
+    g->s[c] = s;
+    g->w[c] = (int)(((long long)f.width * p.h_samp * s + f.max_h * 8 - 1) / (f.max_h * 8));
+    g->h[c] = (int)(((long long)f.height * p.v_samp * s + f.max_v * 8 - 1) / (f.max_v * 8));
+  }
+  for (int c = f.ncomp; c < 3; c++) g->s[c] = g->s[0];
+  return E_OK;
+}
+
+bool JpegScaled::full_chroma() const {
+  for (int c = 0; c < 3; c++)
+    if (w[c] && (w[c] != width || h[c] != height)) return false;
+  return true;
+}
+
 }  // namespace uhdr_b200

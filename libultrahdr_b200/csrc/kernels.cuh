@@ -152,6 +152,20 @@ struct IdctPlaneParams {
   int dst_w, dst_h;                 // samples beyond are not written
 };
 
+// reduced-size IDCT (idct_scaled.cu): the planes of one JPEG whose DCT scaled size is the launch's (4, 2 or 1)
+struct IdctScaledParams {
+  int nplanes;
+  int block_end[3];                 // cumulative block counts: plane i holds blocks [block_end[i-1], block_end[i])
+  struct Plane {
+    const int16_t* coefs;
+    uint16_t q[64];
+    int wblocks;
+    uint8_t* dst;
+    int dst_stride;                 // >= wblocks * size
+    int dst_w, dst_h;               // samples beyond are not written
+  } plane[3];
+};
+
 struct YccToRgbaParams {
   const uint8_t* y; const uint8_t* cb; const uint8_t* cr;
   int src_stride, w, h;
@@ -198,6 +212,7 @@ cudaError_t launch_rgb_to_ycc(const RgbToYccParams& p, cudaStream_t s);
 cudaError_t launch_resize_map(const ResizeMapParams& p, cudaStream_t s);
 cudaError_t launch_fdct8(const Fdct8Params& p, cudaStream_t s);
 cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s);
+cudaError_t launch_idct_scaled(const IdctScaledParams& p, int size, cudaStream_t s);
 cudaError_t launch_ycc_to_rgba(const YccToRgbaParams& p, cudaStream_t s);
 
 // number of kernel launches issued by this library since load (bench.py's gpu_launches)

@@ -73,6 +73,18 @@ def default_gm_config(**kw):
     return c
 
 
+SCALE_DENOMS = (1, 2, 4, 8)  # uhdr_b200_decode_scaled_dev / _jpeg_decode_scaled / _scaled_dims: decode at 1/k
+
+
+def declare_scaled_decode(lib):
+    """argument types of the reduced-size decode entry points (include/uhdr_b200.h) on a loaded libuhdr_b200"""
+    lib.uhdr_b200_scaled_dims.argtypes = [C.c_void_p, C.c_size_t, C.c_int] + [C.POINTER(C.c_uint)] * 4
+    lib.uhdr_b200_decode_scaled_dev.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_float, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.uhdr_b200_jpeg_decode_scaled.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
+    return lib
+
+
 def _ptr(a):
     return None if a is None else a.ctypes.data
 
