@@ -73,11 +73,14 @@ UHDR_EXTERN int uhdr_b200_convert_yuv_dev(uhdr_raw_image_t* image_dev, int src_c
 
 /* JpegEncoderHelper::compressImage, ref lib/src/jpegencoderhelper.cpp:101.  `is_gainmap_comment`
  * is implied by the format exactly as in the reference (RGB888 / Y400 carry the COM marker).
- * out must hold `cap` bytes. */
+ * out must hold `cap` bytes.  Planes whose width is not a multiple of 8 are padded the way the helper pads them for
+ * the given strides: a stride below the 8-aligned width gives columns of 0 (luma) / 128 (chroma) and rows past the
+ * height that repeat the previous iMCU row's; a larger stride reads the caller's bytes up to the aligned width. */
 UHDR_EXTERN int uhdr_b200_jpeg_encode(const uhdr_raw_image_t* img, int quality, const void* icc,
                                       size_t icc_size, void* out, size_t cap, size_t* out_size);
 /* forward block stage only: quantised coefficients per component, raster block order, natural
- * order inside a block (parity hook for FDCT + quantise). coefs[c] sized wblocks*hblocks*64. */
+ * order inside a block (parity hook for FDCT + quantise). coefs[c] sized wblocks*hblocks*64.  Edge padding as in
+ * uhdr_b200_jpeg_encode. */
 UHDR_EXTERN int uhdr_b200_jpeg_forward(const uhdr_raw_image_t* img, int quality, int16_t* coefs[3]);
 /* JpegDecoderHelper::decompressImage, ref lib/src/jpegdecoderhelper.cpp:169.
  * mode: 0 = DECODE_TO_YCBCR_CS raw planes, 1 = DECODE_TO_RGB_CS (RGBA8888), 2 = DECODE_STREAM.
@@ -152,7 +155,8 @@ UHDR_EXTERN int uhdr_b200_encode_dev(const uhdr_raw_image_t* hdr_dev, const uhdr
                                      const void* exif, size_t exif_size,
                                      void* out, size_t cap, size_t* out_size, void* stream);
 /* JpegEncoderHelper::compressImage (ref lib/src/jpegencoderhelper.cpp:101) of a DEVICE image: the formats and
- * bytes of uhdr_b200_jpeg_encode; the stream goes to the HOST buffer out. */
+ * bytes of uhdr_b200_jpeg_encode given zero-initialised rows of 64-pixel aligned stride (the layout uhdr_encode
+ * compresses from; no byte past a row's width is read); the stream goes to the HOST buffer out. */
 UHDR_EXTERN int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img_dev, int quality, const void* icc,
                                           size_t icc_size, void* out, size_t cap, size_t* out_size, void* stream);
 
@@ -196,6 +200,11 @@ UHDR_EXTERN void uhdr_b200_tonemap_stats(unsigned long long out[2]);
  * scales up to 16 and the PQ / HLG outputs), out[2] = k_apply_gainmap (every other input), out[3] = gain-map resizes
  * (aspect ratio off by more than 1 %), each followed by one of the other three. */
 UHDR_EXTERN void uhdr_b200_apply_stats(unsigned long long out[4]);
+/* The encoder's device entropy coder (k_huff_encode) gives each CTA 256 * bpt consecutive blocks of the scan, bpt in
+ * 1..8 being the smallest value that makes the whole grid resident at once (8 beyond 8 waves' worth of blocks).  Plans
+ * since process start, every entry point: out[0] = resident CTAs per wave the plan assumed (0 before the first
+ * encode), out[1..8] = launches with bpt = 1..8, out[9] = launches whose grid exceeded one wave.  Host-side counts. */
+UHDR_EXTERN void uhdr_b200_jpeg_encode_stats(unsigned long long out[10]);
 /* diagnostic: worst[0] = max |approximate pow(e, 1/2.4) - the exact one| over the `count` floats whose bit patterns
  * start at first_bits (the screen relies on <= 3e-7 for e in (0.0031308, 1]; must measure <= 1.5e-7); host pointer. */
 UHDR_EXTERN int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst);

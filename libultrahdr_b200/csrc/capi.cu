@@ -603,10 +603,11 @@ UHDR_API int uhdr_b200_jpeg_forward(const uhdr_raw_image_t* img, int quality, in
   JpegRCodec* c = tls_codec();
   if (!c) return E_ERROR;
   DevImage d;
-  int rc = upload_image(c->ws(), *img, &d);
+  int rows[3];
+  int rc = upload_jpeg_input(c->ws(), *img, &d, rows);
   if (rc) return rc;
   JpegEncodeJob job;
-  rc = jpeg_forward_dev(c->ws(), d, quality, &job);
+  rc = jpeg_forward_dev(c->ws(), d, quality, &job, /*zigzag=*/false, rows);
   if (rc) return rc;
   for (int k = 0; k < job.frame.ncomp; k++)
     CUDA_TRY(cudaMemcpyAsync(coefs[k], job.d_coefs[k], job.frame.blocks(k) * 128, cudaMemcpyDeviceToHost, c->ws().stream()));
@@ -618,9 +619,10 @@ UHDR_API int uhdr_b200_jpeg_encode(const uhdr_raw_image_t* img, int quality, con
   JpegRCodec* c = tls_codec();
   if (!c) return E_ERROR;
   DevImage d;
-  int rc = upload_image(c->ws(), *img, &d);
+  int rows[3];
+  int rc = upload_jpeg_input(c->ws(), *img, &d, rows);
   if (rc) return rc;
-  return compress_image_dev(c->ws(), d, quality, icc, icc_size, /*caller_planes=*/false, (uint8_t*)out, cap, out_size);
+  return compress_image_dev(c->ws(), d, quality, icc, icc_size, /*caller_planes=*/false, (uint8_t*)out, cap, out_size, rows);
 }
 
 static int jpeg_decode_host(const void* data, size_t size, int mode, int k, uhdr_raw_image_t* out, size_t cap) {

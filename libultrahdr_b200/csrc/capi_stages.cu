@@ -83,6 +83,10 @@ UHDR_API void uhdr_b200_apply_stats(unsigned long long out[4]) {
   if (out) apply_route_stats(out);
 }
 
+UHDR_API void uhdr_b200_jpeg_encode_stats(unsigned long long out[10]) {
+  if (out) jpeg_encode_stats(out);
+}
+
 UHDR_API int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst) {
   Workspace* ws = tls_workspace();
   if (!ws || !worst) return E_ERROR;

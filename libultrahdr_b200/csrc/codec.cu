@@ -52,13 +52,57 @@ static int block_stage_input(Workspace& ws, DevImage* img) {
   return upload_image(ws, src, img, cudaMemcpyDeviceToDevice);
 }
 
+// JpegEncoderHelper::compressYCbCr (jpegencoderhelper.cpp:246-309) on a plane whose width is not a multiple of 8:
+//  * stride below the 8-aligned width: each row is staged in a scratch buffer whose columns past the width are 0
+//    (luma) / 128 (chroma); rows past the height are not written, so they keep what the previous iMCU row left in
+//    the scratch rows (0 / 128 in the first one)
+//  * otherwise the columns up to the aligned width are the caller's bytes as they are, rows past the height the pad
+//    row (0 / 128, the block stage's fill)
+// `img` holds the workspace copy of `caller` (zero-tailed); this rebuilds the helper's bytes in it.  rows[c] = rows
+// of plane c the block stage reads from memory (0: up to the height, then the fill).
+static int helper_padding(Workspace& ws, const uhdr_raw_image_t& caller, cudaMemcpyKind kind, const DevImage& img, int rows[3]) {
+  if (img.v.fmt != F_Y400 && img.v.fmt != F_YUV420 && img.v.fmt != F_YUV422 && img.v.fmt != F_YUV444) return E_OK;
+  cudaStream_t st = ws.stream();
+  for (int i = 0; i < fmt_planes(img.v.fmt); i++) {
+    int pw, ph, esz;
+    fmt_plane_geom(img.v.fmt, img.v.w, img.v.h, i, &pw, &ph, &esz);
+    const int aw = (pw + 7) / 8 * 8, fill = i == 0 ? 0 : 128;
+    if (pw == aw || img.v.p[i] == caller.planes[i]) continue;
+    uint8_t* p = (uint8_t*)img.v.p[i];
+    const size_t ds = img.v.stride[i];
+    if ((int)caller.stride[i] >= aw) {
+      CUDA_TRY(cudaMemcpy2DAsync(p + pw, ds, (const uint8_t*)caller.planes[i] + pw, caller.stride[i], aw - pw, ph, kind, st));
+      continue;
+    }
+    CUDA_TRY(cudaMemset2DAsync(p + pw, ds, fill, aw - pw, ph, st));
+    const int imcu = (img.v.fmt == F_YUV420 && i == 0) ? 16 : 8, hb8 = (ph + 7) / 8 * 8;
+    for (int y = ph; y < hb8; y++) {
+      if (y >= imcu) {
+        CUDA_TRY(cudaMemcpyAsync(p + y * ds, p + (y - imcu) * ds, aw, cudaMemcpyDeviceToDevice, st));
+      } else {
+        CUDA_TRY(cudaMemsetAsync(p + y * ds, 0, pw, st));
+        CUDA_TRY(cudaMemsetAsync(p + y * ds + pw, fill, aw - pw, st));
+      }
+    }
+    rows[i] = hb8;
+  }
+  return E_OK;
+}
+
+int upload_jpeg_input(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out, int rows[3]) {
+  rows[0] = rows[1] = rows[2] = 0;
+  int rc = upload_image(ws, src, out);
+  if (rc) return rc;
+  return helper_padding(ws, src, cudaMemcpyHostToDevice, *out, rows);
+}
+
 int compress_image_dev(Workspace& ws, const DevImage& img_in, int quality, const void* icc, size_t icc_size,
-                       bool caller_planes, uint8_t* out, size_t cap, size_t* out_size) {
+                       bool caller_planes, uint8_t* out, size_t cap, size_t* out_size, const int* rows) {
   DevImage img = img_in;
   int rc = caller_planes ? block_stage_input(ws, &img) : E_OK;
   if (rc) return rc;
   JpegEncodeJob job;
-  rc = jpeg_forward_dev(ws, img, quality, &job, /*zigzag=*/true);
+  rc = jpeg_forward_dev(ws, img, quality, &job, /*zigzag=*/true, rows);
   if (rc) return rc;
   rc = jpeg_entropy_dev(ws, &job);
   if (rc) return rc;

@@ -123,8 +123,13 @@ class JpegRCodec {
 
 // JpegEncoderHelper::compressImage (jpegencoderhelper.cpp:101) of a device image, on ws.stream(); returns once the
 // stream is in `out`.  `caller_planes`: see block_stage_input.
+// rows: from upload_jpeg_input (nullptr: the planes are read up to their height, then the pad row)
 int compress_image_dev(Workspace& ws, const DevImage& img, int quality, const void* icc, size_t icc_size,
-                       bool caller_planes, uint8_t* out, size_t cap, size_t* out_size);
+                       bool caller_planes, uint8_t* out, size_t cap, size_t* out_size, const int* rows = nullptr);
+// The input of JpegEncoderHelper::compressImage from HOST planes (uhdr_b200_jpeg_encode, uhdr_b200_jpeg_forward, the
+// C++ JpegEncoderHelper): upload_image, then the helper's edge padding of planes whose width is not a multiple of 8
+// for the caller's strides (jpegencoderhelper.cpp:246-309).  rows[c] goes to jpeg_forward_dev.
+int upload_jpeg_input(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out, int rows[3]);
 
 // uhdr_enc_set_raw_image's checks of one intent's descriptor (ultrahdr_api.cpp:842-1025): its code, the last error
 // set.  The planes are not dereferenced.

@@ -298,9 +298,10 @@ uhdr_error_info_t JpegEncoderHelper::compressImage(const uhdr_raw_image_t* img, 
   if (!c) return from_rc(rc);
   Workspace& ws = c->ws();
   DevImage d;
-  if ((rc = upload_image(ws, *img, &d))) return from_rc(rc);
+  int rows[3];
+  if ((rc = upload_jpeg_input(ws, *img, &d, rows))) return from_rc(rc);
   JpegEncodeJob job;
-  if ((rc = jpeg_forward_dev(ws, d, qfactor, &job, /*zigzag=*/true))) return from_rc(rc);
+  if ((rc = jpeg_forward_dev(ws, d, qfactor, &job, /*zigzag=*/true, rows))) return from_rc(rc);
   if ((rc = jpeg_entropy_dev(ws, &job))) return from_rc(rc);
   if ((rc = ws.sync())) return from_rc(rc);
   if ((rc = jpeg_entropy_fetch(ws, &job))) return from_rc(rc);

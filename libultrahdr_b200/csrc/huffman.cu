@@ -15,6 +15,7 @@
 //   5. byte stuffing folded in: the 0xFF bytes of the words a CTA owns are counted, a second
 //      look-back gives the number of stuffed zeros in front of them, the CTA writes its final bytes
 // Only the final stuffed segment (a few MB at 4K) exists in global memory and crosses PCIe.
+#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -40,11 +41,17 @@ constexpr int kMaxChunk = kEncThreads * kMaxBpt;
 constexpr unsigned kSegWords = 2048;
 constexpr unsigned long long kFlagAgg = 1ull << 62, kFlagPrefix = 2ull << 62, kFlagMask = 3ull << 62;
 
-// floor(n / d) for the small runtime divisors of the scan geometry: one multiply instead of the
-// ~20-instruction integer division.  Exact while n * d < 2^32 (here n < 2^23, d <= 1024).
+// floor(n / d) for the runtime divisors of the scan geometry: a multiply instead of the ~20-instruction
+// integer division.  umulhi(n, ceil(2^32 / d)) is floor(n / d) or one more; the product check takes the
+// excess back.  Exact for n < 2^32 - d (q * d must not wrap); here n < 2^27.  Needed: MCUs per row reach
+// 8191 (a Y400 frame 65535 wide), so n * d passes 2^32 and the multiply alone is off by one.
 struct FastDiv {
   unsigned d, m;  // m = ceil(2^32 / d); d == 1 is flagged with m = 0
-  __device__ __forceinline__ unsigned div(unsigned n) const { return m ? __umulhi(n, m) : n; }
+  __device__ __forceinline__ unsigned div(unsigned n) const {
+    if (!m) return n;
+    const unsigned q = __umulhi(n, m);
+    return q * d > n ? q - 1 : q;
+  }
 };
 
 struct HuffFrame {
@@ -497,8 +504,14 @@ static int device_books(const uint32_t** out) {
   return E_OK;
 }
 
+// what jpeg_entropy_dev planned: resident CTAs per wave, launches by bpt (index 1..8), launches beyond one wave
+std::atomic<unsigned long long> g_enc_plan[10];
+
 }  // namespace
 
+void jpeg_encode_stats(unsigned long long out[10]) {
+  for (int i = 0; i < 10; i++) out[i] = g_enc_plan[i].load(std::memory_order_relaxed);
+}
 
 int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job) {
   const JpegFrame& fr = job->frame;
@@ -566,6 +579,9 @@ int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job) {
     if (trace) cudaMemsetAsync(trace, 0, (size_t)ncta * 16 * 8, st);
   }
   k_huff_encode<<<ncta, kEncThreads, 0, st>>>(f, books, status, ffstatus, tails, job->d_scan, (unsigned)cap, ctl, trace);
+  g_enc_plan[0].store((unsigned long long)resident, std::memory_order_relaxed);
+  g_enc_plan[bpt].fetch_add(1, std::memory_order_relaxed);
+  if (ncta > (unsigned)resident) g_enc_plan[9].fetch_add(1, std::memory_order_relaxed);
   if (trace) {
     std::vector<unsigned long long> h((size_t)ncta * 16);
     cudaMemcpyAsync(h.data(), trace, h.size() * 8, cudaMemcpyDeviceToHost, st);

@@ -55,11 +55,17 @@ struct JpegEncodeJob {
 // Enqueue the block stage for `img` (device image): colour conversion (RGB888 only), level
 // shift, FDCT, quantise.  Mirrors JpegEncoderHelper::compressImage's input handling
 // (jpegencoderhelper.cpp:131-309) including libjpeg's edge rules.
-int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag = false);
+// rows[c] > 0: the block stage reads rows [0, rows[c]) of plane c from memory (the encoder helper's scratch rows),
+// not only those up to the plane height
+int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag = false,
+                     const int* rows = nullptr);
 // Enqueue entropy coding on the device + async copy of the scan to pinned memory.
 int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job);
 // second phase, once the stream was synchronised and the sizes are on the host
 int jpeg_entropy_fetch(Workspace& ws, JpegEncodeJob* job);
+// k_huff_encode plans since process start: [0] resident CTAs per wave, [1..8] launches by blocks per thread,
+// [9] launches whose grid exceeded one wave
+void jpeg_encode_stats(unsigned long long out[10]);
 // After stream sync: assemble SOI..EOI.  `comment` != nullptr adds the COM marker the reference
 // writes for gain-map images (jpegencoderhelper.cpp:205-211).
 int jpeg_finish_stream(const JpegEncodeJob& job, const void* icc, size_t icc_size,

@@ -7,7 +7,7 @@
 
 namespace uhdr_b200 {
 
-int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag) {
+int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag, const int* rows) {
   int rc = jpeg_frame_init(&job->frame, img.v.fmt, img.v.w, img.v.h, quality);
   if (rc) return rc;
   const JpegFrame& f = job->frame;
@@ -62,7 +62,7 @@ int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncode
       pl.src = (const uint8_t*)img.v.p[c];
       pl.stride = img.v.stride[c];
       pl.w = k.wblocks * 8;
-      pl.h = k.height;
+      pl.h = rows && rows[c] > 0 ? rows[c] : k.height;
       pl.wblocks = k.wblocks;
       pl.hblocks = k.hblocks;
       pl.fill = c == 0 ? 0 : 128;

@@ -85,6 +85,20 @@ def declare_scaled_decode(lib):
     return lib
 
 
+def declare_jpeg_encode_stats(lib):
+    """uhdr_b200_jpeg_encode_stats(unsigned long long out[10]) on a loaded libuhdr_b200"""
+    lib.uhdr_b200_jpeg_encode_stats.argtypes = [C.POINTER(C.c_ulonglong)]
+    lib.uhdr_b200_jpeg_encode_stats.restype = None
+    return lib
+
+
+def jpeg_encode_stats(lib):
+    """-> (resident CTAs per wave, (launches with bpt 1..8), launches beyond one wave)"""
+    st = (C.c_ulonglong * 10)()
+    lib.uhdr_b200_jpeg_encode_stats(st)
+    return st[0], tuple(st[1:9]), st[9]
+
+
 def _ptr(a):
     return None if a is None else a.ctypes.data
 

@@ -142,6 +142,29 @@ int main(int argc, char** argv) {
     CHECK(st.error_code == UHDR_CODEC_OK);
     printf("sdrjpg %zu %016llx\n", enc.getCompressedImageSize(), (unsigned long long)fnv(enc.getCompressedImagePtr(), enc.getCompressedImageSize()));
   }
+  // widths that are not a multiple of 8: the helper's edge padding for tight strides (0 / 128 columns, rows below the
+  // image repeated from the previous iMCU row) and for wide ones (the caller's bytes up to the aligned width)
+  for (int wide = 0; wide < 2; wide++) {
+    const int w = 246, h = 26;
+    std::vector<uint8_t> tight((size_t)w * h + 2 * (size_t)(w / 2) * (h / 2));
+    for (int y = 0; y < h; y++) memcpy(tight.data() + (size_t)y * w, yuvbuf.data() + (size_t)y * kW, w);
+    for (int c = 0; c < 2; c++)
+      for (int y = 0; y < h / 2; y++)
+        memcpy(tight.data() + (size_t)w * h + (size_t)c * (w / 2) * (h / 2) + (size_t)y * (w / 2),
+               yuvbuf.data() + (size_t)kW * kH + (size_t)c * (kW / 2) * (kH / 2) + (size_t)y * (kW / 2), w / 2);
+    const uint8_t* planes[3] = {tight.data(), tight.data() + (size_t)w * h, tight.data() + (size_t)w * h + (size_t)(w / 2) * (h / 2)};
+    const unsigned strides[3] = {(unsigned)w, (unsigned)w / 2, (unsigned)w / 2};
+    const uint8_t* wplanes[3] = {yuvbuf.data(), yuvbuf.data() + (size_t)kW * kH, yuvbuf.data() + (size_t)kW * kH * 5 / 4};
+    const unsigned wstrides[3] = {(unsigned)kW, (unsigned)kW / 2, (unsigned)kW / 2};
+    for (int fmt = 0; fmt < 2; fmt++) {
+      JpegEncoderHelper e;
+      uhdr_error_info_t st = e.compressImage(wide ? wplanes : planes, wide ? wstrides : strides, w - (fmt ? 1 : 0), h - (fmt ? 5 : 0),
+                                             fmt ? UHDR_IMG_FMT_8bppYCbCr400 : UHDR_IMG_FMT_12bppYCbCr420, kQuality, nullptr, 0);
+      CHECK(st.error_code == UHDR_CODEC_OK);
+      printf("ragged %s %s %zu %016llx\n", wide ? "wide" : "tight", fmt ? "y400" : "420", e.getCompressedImageSize(),
+             (unsigned long long)fnv(e.getCompressedImagePtr(), e.getCompressedImageSize()));
+    }
+  }
   jpegr_compressed_struct sdrjpg;
   sdrjpg.data = enc.getCompressedImagePtr();
   sdrjpg.length = sdrjpg.maxLength = enc.getCompressedImageSize();

@@ -81,7 +81,19 @@ def test_8k_uhdr_decode(gpu, oracle_libs):
     ref = _need_ref(oracle_libs)
     mine = T.UhdrApi(gpu.lib)
     hdr, sdr, keep = _bench_frame(7680, 4320, 7)
+    A.declare_jpeg_encode_stats(gpu.lib)
+    _, b0, _ = A.jpeg_encode_stats(gpu.lib)
     data = mine.encode(hdr, sdr)
+    R, b1, _ = A.jpeg_encode_stats(gpu.lib)
+    # the GPU-encoded file itself == the reference's.  Its two scans go through the entropy coder with the blocks per
+    # thread of their sizes (4:2:0 base 777600 blocks, 3-channel map 1555200: bpt 4 and 8 at 792 resident CTAs)
+    grew = [y - x for x, y in zip(b0, b1)]
+    want_grew = [0] * 8
+    for n in (777600, 1555200):
+        want_grew[min(8, -(-n // (256 * R))) - 1] += 1
+    assert grew == want_grew, (R, grew)
+    want = ref.encode(hdr, sdr)
+    assert len(data) == len(want) and data == want
     st0, st1 = (C.c_ulonglong * 3)(), (C.c_ulonglong * 3)()
     gpu.lib.uhdr_b200_entropy_decoder_stats.restype = None
     gpu.lib.uhdr_b200_entropy_decoder_stats(st0)

@@ -37,12 +37,14 @@ SIZES = {A.FMT_YUV420: [(64, 48), (320, 240), (1280, 720)],
          A.FMT_Y400: [(64, 48), (320, 180), (960, 540), (72, 33)],
          A.FMT_RGB888: [(64, 48), (320, 180), (100, 61), (960, 540)],
          A.FMT_YUV444: [(64, 48), (96, 40)]}
+# widths that are not a multiple of 8 with tight strides: the encoder pads them the way its helper does
+ENCODE_SIZES = {f: s + {A.FMT_YUV420: [(246, 26)], A.FMT_Y400: [(261, 37)]}.get(f, []) for f, s in SIZES.items()}
 
 
 @pytest.mark.parametrize("fmt", list(SIZES))
 def test_forward_coefficients(gpu, oracle_libs, fmt):
     o = oracle_libs.Oracle().lib
-    for (w, h) in SIZES[fmt]:
+    for (w, h) in ENCODE_SIZES[fmt]:
         for kind, q in (("noise", 95), ("smooth", 50), ("noise", 100), ("smooth", 7)):
             img, keep = _img(fmt, w, h, kind)
             f, ref = T.oracle_forward(o, img, q)
@@ -55,7 +57,7 @@ def test_forward_coefficients(gpu, oracle_libs, fmt):
 def test_encode_stream_bytes(gpu, oracle_libs, fmt):
     o = oracle_libs.Oracle().lib
     icc = bytes(range(40))
-    for (w, h) in SIZES[fmt]:
+    for (w, h) in ENCODE_SIZES[fmt]:
         for kind, q in (("noise", 95), ("smooth", 85)):
             img, keep = _img(fmt, w, h, kind)
             gm = fmt in (A.FMT_RGB888, A.FMT_Y400)
