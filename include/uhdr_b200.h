@@ -145,6 +145,39 @@ UHDR_EXTERN int uhdr_b200_decode_scaled_dev(const void* data, size_t size, int k
  * gives RGBA8888 at that size. */
 UHDR_EXTERN int uhdr_b200_jpeg_decode_scaled(const void* data, size_t size, int mode, int k, uhdr_raw_image_t* out,
                                              size_t cap);
+/* A JPEG/R decoded once and kept in device memory, then rendered at any display boost, output transfer and viewport
+ * without decoding again: a viewer re-renders as the display's headroom or the visible rectangle changes, a server
+ * renders one upload as linear, HLG and PQ.  A render costs one apply kernel (or, for SRGB, one colour conversion)
+ * over the rectangle plus a table upload of a few KB.
+ *
+ * uhdr_b200_image_open_dev: decodes both JPEGs of the file at 1/k (k in {1, 2, 4, 8}, as uhdr_b200_decode_scaled_dev)
+ * on the current device, to which the image stays bound.  It keeps the primary image's YCbCr planes, the decoded gain
+ * map (resized once, here, when its aspect ratio differs from the primary image's by more than 1 %, as applyGainMap
+ * would on every call), the metadata and the gamuts; the entropy decoder's scratch is not kept.  Returns when the
+ * image is resident.  Errors: those of uhdr_b200_decode_scaled_dev on the same file (corrupt data, no metadata, a k
+ * outside {1, 2, 4, 8}, 4:2:2 / 4:4:0 / 4:1:1 at k > 1); a gray primary image gives UHDR_CODEC_UNSUPPORTED_FEATURE.
+ * Without a device: UHDR_CODEC_ERROR with a CUDA message.  *out is NULL after a failure.
+ * uhdr_b200_image_info: the 1/k primary image's *w x *h, the decoded gain map's *gm_w x *gm_h (both as
+ * uhdr_b200_scaled_dims gives them), the metadata and the device memory the image holds.  Any pointer may be NULL.
+ * uhdr_b200_image_render_dev: writes the dest_dev->w x dest_dev->h pixels of the image that start at (x, y) into
+ * dest_dev.  The bytes equal that rectangle cut from uhdr_b200_decode_scaled_dev's result for the same k, out_ct,
+ * max_display_boost and format (for k = 1 also from uhdr_b200_decode_dev's and uhdr_decode's).  dest_dev follows the
+ * decode_dev rules above: fmt / out_ct pair as there, planes[0] device memory of the image's device aligned to a
+ * pixel, any stride >= w, the bytes past a row's width untouched; on success cg / ct / range are set as decode_dev sets
+ * them.  The rectangle must be non-empty and inside the image.  Stream order: the writes follow the work enqueued
+ * earlier on `stream` and are visible to later work on it; the call does not wait on the host, except when all of the
+ * image's few per-render table slots are still in use by renders in flight.  Renders may go to different streams.  A
+ * failing call writes nothing; bad arguments give UHDR_CODEC_INVALID_PARAM.  An image is not thread-safe (one host
+ * thread at a time), distinct images are independent.
+ * uhdr_b200_image_release: waits for the image's outstanding renders, then returns its memory to the process-wide
+ * cache of released handles (uhdr_b200_trim_cache). */
+typedef struct uhdr_b200_image uhdr_b200_image_t;
+UHDR_EXTERN int uhdr_b200_image_open_dev(const void* data, size_t size, int k, uhdr_b200_image_t** out);
+UHDR_EXTERN int uhdr_b200_image_info(const uhdr_b200_image_t* img, unsigned* w, unsigned* h, unsigned* gm_w,
+                                     unsigned* gm_h, uhdr_gainmap_metadata_t* md, size_t* device_bytes);
+UHDR_EXTERN int uhdr_b200_image_render_dev(uhdr_b200_image_t* img, int out_ct, float max_display_boost, unsigned x,
+                                           unsigned y, uhdr_raw_image_t* dest_dev, void* stream);
+UHDR_EXTERN int uhdr_b200_image_release(uhdr_b200_image_t* img);
 /* JpegR::encodeJPEGR API-1 (sdr_dev != NULL, ref lib/src/jpegr.cpp:247-291) / API-0 (sdr_dev == NULL, :179-244)
  * from intents in device memory.  The JPEG/R file is written to the HOST buffer out (cap bytes); *out_size
  * receives its length.  The bytes equal uhdr_encode's for the same intents and settings: cfg carries the settings

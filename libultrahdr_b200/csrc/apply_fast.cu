@@ -80,7 +80,9 @@ __device__ __forceinline__ int idx1023(float x) {  // x >= 0: int32(double(x*102
   return (__float2int_rz(x * 2046.0f) + 1) >> 1;
 }
 
-template <int BPP, bool SCALE1, int GAMUT /*0 none 1 sdr side 2 hdr side*/, int OUT /*0 F16 1 PQ 2 HLG*/>
+// ORG: a region whose origin (p.ox, p.oy) is not 0, 0 (x, y below are relative to it); false compiles to the
+// whole-image kernel
+template <int BPP, bool SCALE1, int GAMUT /*0 none 1 sdr side 2 hdr side*/, int OUT /*0 F16 1 PQ 2 HLG*/, bool ORG>
 __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyParams p, const float* __restrict__ gain_u8) {
   extern __shared__ float smem_raw[];
   FastSmem& sm = *reinterpret_cast<FastSmem*>(smem_raw);
@@ -98,17 +100,19 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyPara
   __syncthreads();
   const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (x >= p.sdr.w) return;
+  const int ax = ORG ? p.ox + x : x;   // absolute column of the reads (ox % 4 == 0, oy % 2 == 0)
   const uint8_t* __restrict__ Y = (const uint8_t*)p.sdr.p[0];
   const int ybase = blockIdx.y * (kBlockY * kRowsPerThread) + threadIdx.y * 2;
 #pragma unroll 1
   for (int it = 0; it < kRowsPerThread / 2; it++) {
   const int y = ybase + it * (kBlockY * 2);
   if (y >= p.sdr.h) break;
-  const unsigned y0 = __ldg((const unsigned*)(Y + (size_t)y * p.sdr.stride[0] + x));
-  const unsigned y1 = __ldg((const unsigned*)(Y + (size_t)(y + 1) * p.sdr.stride[0] + x));
-  const size_t coff = (size_t)(y >> 1) * p.sdr.stride[1] + (x >> 1);
+  const int ay = ORG ? p.oy + y : y;
+  const unsigned y0 = __ldg((const unsigned*)(Y + (size_t)ay * p.sdr.stride[0] + ax));
+  const unsigned y1 = __ldg((const unsigned*)(Y + (size_t)(ay + 1) * p.sdr.stride[0] + ax));
+  const size_t coff = (size_t)(ay >> 1) * p.sdr.stride[1] + (ax >> 1);
   const unsigned uu = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[1] + coff));
-  const unsigned vv = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[2] + (size_t)(y >> 1) * p.sdr.stride[2] + (x >> 1)));
+  const unsigned vv = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[2] + (size_t)(ay >> 1) * p.sdr.stride[2] + (ax >> 1)));
   // chroma terms of p3YuvToRgb, shared by the 2x2 pixels under each chroma sample
   float crv[2], gcbu[2], gcrv[2], cbu[2];
 #pragma unroll
@@ -123,13 +127,13 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyPara
 #pragma unroll
   for (int r = 0; r < 2; r++) {
     const unsigned yw = r ? y1 : y0;
-    const int yy = y + r;
+    const int yy = y + r, ayy = ay + r;
     unsigned out[8];
     // gain-map taps for the 4 pixels of this row
     uint4 m4 = make_uint4(0, 0, 0, 0);
     unsigned m3[3] = {0, 0, 0};
     if (SCALE1) {
-      const uint8_t* mrow = p.map + ((size_t)yy * p.map_stride + x) * BPP;
+      const uint8_t* mrow = p.map + ((size_t)ayy * p.map_stride + ax) * BPP;
       if (BPP == 4) m4 = __ldg((const uint4*)mrow);
       else if (BPP == 3) { m3[0] = __ldg((const unsigned*)mrow); m3[1] = __ldg((const unsigned*)mrow + 1); m3[2] = __ldg((const unsigned*)mrow + 2); }
       else m3[0] = __ldg((const unsigned*)mrow);
@@ -170,8 +174,8 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyPara
         fb = BPP == 1 ? fr : *reinterpret_cast<const float*>(gt + 2048 + o2);
       } else {
         const int s = p.scale_int;
-        const int px = x + i;
-        int xl = px / s, yl = yy / s;
+        const int px = ax + i;
+        int xl = px / s, yl = ayy / s;
         const int xu = min(xl + 1, p.map_w - 1), yu = min(yl + 1, p.map_h - 1);
         xl = min(xl, p.map_w - 1);
         yl = min(yl, p.map_h - 1);
@@ -179,7 +183,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY) k_apply_fast(const ApplyPara
         if (xl == xu && yl == yu) variant = 3;
         else if (xl == xu) variant = 1;
         else if (yl == yu) variant = 2;
-        const float* w = idw + (variant * s * s + (yy % s) * s + (px % s)) * 4;
+        const float* w = idw + (variant * s * s + (ayy % s) * s + (px % s)) * 4;
         const float w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3];
         const uint8_t* m = p.map;
         const size_t i1 = ((size_t)yl * p.map_stride + xl) * BPP, i2 = ((size_t)yu * p.map_stride + xl) * BPP;
@@ -288,7 +292,7 @@ struct TileIn {   // what one thread reads for its 4x2 pixels
   int x, y;
 };
 
-template <int BPP, int GAMUT, bool NANS>
+template <int BPP, int GAMUT, bool NANS, bool ORG>
 __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyParams p, const float* __restrict__ gain_u8, const int tiles_x,
                                                                  const int ntiles, const unsigned long long nz,
                                                                  unsigned* __restrict__ sched) {
@@ -323,15 +327,16 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyP
     const int x = (tx * kBlockX + threadIdx.x) * 4;
     const int y = ty * (kBlockY * 2) + threadIdx.y * 2;
     if (x >= p.sdr.w || y >= p.sdr.h) return false;
-    in.x = x;
+    in.x = x;   // stores: relative to the region
     in.y = y;
-    in.yw[0] = __ldg((const unsigned*)(Y + (size_t)y * p.sdr.stride[0] + x));
-    in.yw[1] = __ldg((const unsigned*)(Y + (size_t)(y + 1) * p.sdr.stride[0] + x));
-    in.uu = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[1] + (size_t)(y >> 1) * p.sdr.stride[1] + (x >> 1)));
-    in.vv = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[2] + (size_t)(y >> 1) * p.sdr.stride[2] + (x >> 1)));
+    const int ax = ORG ? p.ox + x : x, ay = ORG ? p.oy + y : y;   // reads: absolute
+    in.yw[0] = __ldg((const unsigned*)(Y + (size_t)ay * p.sdr.stride[0] + ax));
+    in.yw[1] = __ldg((const unsigned*)(Y + (size_t)(ay + 1) * p.sdr.stride[0] + ax));
+    in.uu = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[1] + (size_t)(ay >> 1) * p.sdr.stride[1] + (ax >> 1)));
+    in.vv = __ldg((const uint16_t*)((const uint8_t*)p.sdr.p[2] + (size_t)(ay >> 1) * p.sdr.stride[2] + (ax >> 1)));
 #pragma unroll
     for (int r = 0; r < 2; r++) {
-      const uint8_t* mrow = p.map + ((size_t)(y + r) * p.map_stride + x) * BPP;
+      const uint8_t* mrow = p.map + ((size_t)(ay + r) * p.map_stride + ax) * BPP;
       if (BPP == 4) in.m4[r] = __ldg((const uint4*)mrow);
       else if (BPP == 3) { in.m3[r][0] = __ldg((const unsigned*)mrow); in.m3[r][1] = __ldg((const unsigned*)mrow + 1); in.m3[r][2] = __ldg((const unsigned*)mrow + 2); }
       else in.m3[r][0] = __ldg((const unsigned*)mrow);
@@ -445,7 +450,7 @@ __global__ void __launch_bounds__(kBlockX* kBlockY, 4) k_apply_lin1(const ApplyP
   }
 }
 
-template <int BPP, bool NANS>
+template <int BPP, bool NANS, bool ORG>
 cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sched, cudaStream_t s) {
   const int tiles_x = (p.sdr.w / 4 + kBlockX - 1) / kBlockX, tiles_y = (p.sdr.h + kBlockY * 2 - 1) / (kBlockY * 2);
   const int ntiles = tiles_x * tiles_y;
@@ -455,8 +460,8 @@ cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sc
   static int resident[3] = {0, 0, 0};
   if (!resident[g]) {
     int per_sm = 0, dev = 0, sms = 0;
-    const void* fn = g == 0 ? (const void*)k_apply_lin1<BPP, 0, NANS> : g == 1 ? (const void*)k_apply_lin1<BPP, 1, NANS>
-                                                                         : (const void*)k_apply_lin1<BPP, 2, NANS>;
+    const void* fn = g == 0 ? (const void*)k_apply_lin1<BPP, 0, NANS, ORG> : g == 1 ? (const void*)k_apply_lin1<BPP, 1, NANS, ORG>
+                                                                              : (const void*)k_apply_lin1<BPP, 2, NANS, ORG>;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlockX * kBlockY, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
@@ -464,29 +469,46 @@ cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sc
   }
   int ctas = resident[g];
   if (ctas > ntiles) ctas = ntiles;
-  if (g == 0) k_apply_lin1<BPP, 0, NANS><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
-  else if (g == 1) k_apply_lin1<BPP, 1, NANS><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
-  else k_apply_lin1<BPP, 2, NANS><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  if (g == 0) k_apply_lin1<BPP, 0, NANS, ORG><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  else if (g == 1) k_apply_lin1<BPP, 1, NANS, ORG><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
+  else k_apply_lin1<BPP, 2, NANS, ORG><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
   return cudaGetLastError();
 }
-template <int BPP>
+template <int BPP, bool ORG>
 cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sched, cudaStream_t s) {
-  return p.nan_possible ? launch_lin1<BPP, true>(p, gain_u8, sched, s) : launch_lin1<BPP, false>(p, gain_u8, sched, s);
+  return p.nan_possible ? launch_lin1<BPP, true, ORG>(p, gain_u8, sched, s) : launch_lin1<BPP, false, ORG>(p, gain_u8, sched, s);
 }
 
-template <int BPP, bool S1, int G>
+template <int BPP, bool S1, int G, bool ORG>
 cudaError_t launch_out(const ApplyParams& p, const float* gain_u8, dim3 grid, dim3 block, size_t smem, cudaStream_t s) {
-  if (p.out_ct == CT_LINEAR) k_apply_fast<BPP, S1, G, 0><<<grid, block, smem, s>>>(p, gain_u8);
-  else if (p.out_ct == CT_PQ) k_apply_fast<BPP, S1, G, 1><<<grid, block, smem, s>>>(p, gain_u8);
-  else k_apply_fast<BPP, S1, G, 2><<<grid, block, smem, s>>>(p, gain_u8);
+  if (p.out_ct == CT_LINEAR) k_apply_fast<BPP, S1, G, 0, ORG><<<grid, block, smem, s>>>(p, gain_u8);
+  else if (p.out_ct == CT_PQ) k_apply_fast<BPP, S1, G, 1, ORG><<<grid, block, smem, s>>>(p, gain_u8);
+  else k_apply_fast<BPP, S1, G, 2, ORG><<<grid, block, smem, s>>>(p, gain_u8);
   return cudaGetLastError();
 }
-template <int BPP, bool S1>
+template <int BPP, bool S1, bool ORG>
 cudaError_t launch_gamut(const ApplyParams& p, const float* gain_u8, dim3 grid, dim3 block, size_t smem, cudaStream_t s) {
   const int g = p.gamut_identity ? 0 : (p.gamut_on_sdr ? 1 : 2);
-  if (g == 0) return launch_out<BPP, S1, 0>(p, gain_u8, grid, block, smem, s);
-  if (g == 1) return launch_out<BPP, S1, 1>(p, gain_u8, grid, block, smem, s);
-  return launch_out<BPP, S1, 2>(p, gain_u8, grid, block, smem, s);
+  if (g == 0) return launch_out<BPP, S1, 0, ORG>(p, gain_u8, grid, block, smem, s);
+  if (g == 1) return launch_out<BPP, S1, 1, ORG>(p, gain_u8, grid, block, smem, s);
+  return launch_out<BPP, S1, 2, ORG>(p, gain_u8, grid, block, smem, s);
+}
+
+template <bool ORG>
+cudaError_t launch_fast(const ApplyParams& p, const float* gain_u8, cudaStream_t s) {
+  dim3 block(kBlockX, kBlockY);
+  dim3 grid((p.sdr.w / 4 + kBlockX - 1) / kBlockX, (p.sdr.h + kBlockY * kRowsPerThread - 1) / (kBlockY * kRowsPerThread));
+  const bool s1 = p.scale_int == 1;
+  if (s1 && p.out_ct == CT_LINEAR) {
+    unsigned* sched = reinterpret_cast<unsigned*>(const_cast<float*>(gain_u8) + 768);  // zeroed with the upload
+    if (p.map_bpp == 4) return launch_lin1<4, ORG>(p, gain_u8, sched, s);
+    if (p.map_bpp == 3) return launch_lin1<3, ORG>(p, gain_u8, sched, s);
+    return launch_lin1<1, ORG>(p, gain_u8, sched, s);
+  }
+  const size_t smem = sizeof(FastSmem) + (s1 ? 0 : sizeof(float) * 16 * p.scale_int * p.scale_int);
+  if (p.map_bpp == 4) return s1 ? launch_gamut<4, true, ORG>(p, gain_u8, grid, block, smem, s) : launch_gamut<4, false, ORG>(p, gain_u8, grid, block, smem, s);
+  if (p.map_bpp == 3) return s1 ? launch_gamut<3, true, ORG>(p, gain_u8, grid, block, smem, s) : launch_gamut<3, false, ORG>(p, gain_u8, grid, block, smem, s);
+  return s1 ? launch_gamut<1, true, ORG>(p, gain_u8, grid, block, smem, s) : launch_gamut<1, false, ORG>(p, gain_u8, grid, block, smem, s);
 }
 
 }  // namespace
@@ -495,11 +517,12 @@ bool apply_fast_eligible(const ApplyParams& p) {
   if (p.sdr.fmt != F_YUV420 || !p.scale_int) return false;
   if (p.gamma_inv[0] != 1.0f || p.gamma_inv[1] != 1.0f || p.gamma_inv[2] != 1.0f) return false;
   if ((p.sdr.w & 3) || (p.sdr.h & 1)) return false;
+  if ((p.ox & 3) || (p.oy & 1)) return false;   // a region keeps the 4x2 tiles on the chroma grid and the loads aligned
   if ((p.sdr.stride[0] & 3) || (p.sdr.stride[1] & 1) || (p.sdr.stride[2] & 1)) return false;
   if (((size_t)p.sdr.p[0] & 3) || ((size_t)p.sdr.p[1] & 1) || ((size_t)p.sdr.p[2] & 1)) return false;
   if (((size_t)p.dst & 15) || (p.dst_stride & 3)) return false;
   if (p.scale_int == 1) {
-    if (p.map_w < p.sdr.w || p.map_h < p.sdr.h) return false;  // no edge clamping in the vector path
+    if (p.map_w < p.ox + p.sdr.w || p.map_h < p.oy + p.sdr.h) return false;  // no edge clamping in the vector path
     const int row_bytes = p.map_stride * p.map_bpp;
     if ((row_bytes & 3) || ((size_t)p.map & 15) || (p.map_bpp == 4 && (row_bytes & 15))) return false;
   } else if (p.scale_int > 16) {
@@ -512,19 +535,7 @@ bool apply_fast_eligible(const ApplyParams& p) {
 // (tile counter of the persistent kernel)
 cudaError_t launch_apply_fast(const ApplyParams& p, const float* gain_u8, cudaStream_t s) {
   count_launches(1);
-  dim3 block(kBlockX, kBlockY);
-  dim3 grid((p.sdr.w / 4 + kBlockX - 1) / kBlockX, (p.sdr.h + kBlockY * kRowsPerThread - 1) / (kBlockY * kRowsPerThread));
-  const bool s1 = p.scale_int == 1;
-  if (s1 && p.out_ct == CT_LINEAR) {
-    unsigned* sched = reinterpret_cast<unsigned*>(const_cast<float*>(gain_u8) + 768);  // zeroed with the upload
-    if (p.map_bpp == 4) return launch_lin1<4>(p, gain_u8, sched, s);
-    if (p.map_bpp == 3) return launch_lin1<3>(p, gain_u8, sched, s);
-    return launch_lin1<1>(p, gain_u8, sched, s);
-  }
-  const size_t smem = sizeof(FastSmem) + (s1 ? 0 : sizeof(float) * 16 * p.scale_int * p.scale_int);
-  if (p.map_bpp == 4) return s1 ? launch_gamut<4, true>(p, gain_u8, grid, block, smem, s) : launch_gamut<4, false>(p, gain_u8, grid, block, smem, s);
-  if (p.map_bpp == 3) return s1 ? launch_gamut<3, true>(p, gain_u8, grid, block, smem, s) : launch_gamut<3, false>(p, gain_u8, grid, block, smem, s);
-  return s1 ? launch_gamut<1, true>(p, gain_u8, grid, block, smem, s) : launch_gamut<1, false>(p, gain_u8, grid, block, smem, s);
+  return (p.ox | p.oy) ? launch_fast<true>(p, gain_u8, s) : launch_fast<false>(p, gain_u8, s);
 }
 
 }  // namespace uhdr_b200

@@ -316,7 +316,8 @@ UHDR_API int uhdr_b200_convert_yuv_dev(uhdr_raw_image_t* image, int src_cg, int 
 }
 
 // ---- whole-file codec on device images -------------------------------------------------------------------
-namespace {
+}  // extern "C"
+namespace uhdr_b200 {
 // One codec per host thread and device (a handle is bound to the device that was current when it was made): a
 // decode needs its second workspace and parked helper thread.  settle() first: an earlier decode's writes into a
 // caller's planes may still read this codec's scratch.
@@ -369,6 +370,9 @@ int check_dev_memory(const uhdr_raw_image_t& img, const char* what) {
   }
   return E_OK;
 }
+}  // namespace uhdr_b200
+extern "C" {
+namespace {
 bool valid_scale(int k) { return k == 1 || k == 2 || k == 4 || k == 8; }
 // the probed sizes at 1/k: libjpeg's output size of a scale_denom = k decode, ceil(size / k)
 void scale_dims(DecodedInfo* info, int k) {

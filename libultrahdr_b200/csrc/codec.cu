@@ -485,6 +485,7 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     p.c_stride = strides[1];
     p.cw = (p.w + p.hs - 1) / p.hs;
     p.ch = (p.h + p.vs - 1) / p.vs;
+    p.ox = p.oy = 0;
     if (to_rgba) {
       *to_rgba = p;
       return E_OK;
@@ -549,6 +550,61 @@ int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt
   return rc;
 }
 
+int JpegRCodec::decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go, size_t gl, int sdr_mode,
+                            YccToRgbaParams* to_rgba, bool want_map, int k, DevImage* sdr, DevImage* map, JpegHeader* ph,
+                            JpegHeader* gh, PhaseTrace& tr) {
+  int rc = E_OK;
+  // both images sizeable: the gain-map JPEG goes to a helper thread with its own stream
+  const bool overlap = want_map && pl >= (256u << 10) && gl >= (256u << 10);
+  struct MapJob {   // lives on this frame until helper_.wait() below
+    JpegRCodec* self;
+    const uint8_t* data;
+    size_t len;
+    DevImage* map;
+    JpegHeader* gh;
+    int dev, k, rc;
+    char err[256];
+  } mj{this, data + go, gl, map, gh, 0, k, E_OK, {0}};
+  if (overlap) {
+    if (!ws2_) {
+      ws2_.reset(new Workspace());
+      rc = ws2_->init();
+      if (rc) { ws2_.reset(); return rc; }
+      CUDA_TRY(cudaEventCreateWithFlags(&map_ready_, cudaEventDisableTiming));
+    }
+    ws2_->rewind();
+    CUDA_TRY(cudaGetDevice(&mj.dev));
+    helper_.start([](void* a) {
+      MapJob& j = *static_cast<MapJob*>(a);
+      auto fail_with = [&](int rc, const char* what) { j.rc = rc; snprintf(j.err, sizeof j.err, "%s", what); };
+      if (cudaSetDevice(j.dev) != cudaSuccess) return fail_with(E_ERROR, "cudaSetDevice failed in the gain-map decode thread");
+      j.rc = j.self->decode_jpeg_dev(*j.self->ws2_, j.data, j.len, 2, j.map, j.gh, nullptr, j.k);  // DECODE_STREAM :1486
+      if (j.rc) snprintf(j.err, sizeof j.err, "%s", last_error());
+      else if (cudaEventRecord(j.self->map_ready_, j.self->ws2_->stream()) != cudaSuccess) fail_with(E_ERROR, "cudaEventRecord failed");
+    }, &mj);
+  }
+  rc = decode_jpeg_dev(ws_, data + po, pl, sdr_mode, sdr, ph, to_rgba, k);
+  if (overlap) helper_.wait();
+  if (rc) return rc;
+  tr.mark("primary jpeg enqueued");
+  ByteView blob = find_marker(data + po, *ph, 0xE2, "ICC_PROFILE", 12);
+  sdr->cg = icc_read_gamut(blob.data, blob.size);
+  if (want_map) {
+    if (overlap) {
+      if (mj.rc) { set_last_error(mj.err); return mj.rc; }
+      CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), map_ready_, 0));
+      if (kernel_timing_enabled()) ws2_->sync();
+    } else {
+      rc = decode_jpeg_dev(ws_, data + go, gl, 2, map, gh, nullptr, k);  // DECODE_STREAM :1486
+      if (rc) return rc;
+    }
+    blob = find_marker(data + go, *gh, 0xE2, "ICC_PROFILE", 12);
+    map->cg = icc_read_gamut(blob.data, blob.size);
+    tr.mark("gainmap jpeg enqueued");
+  }
+  return E_OK;
+}
+
 int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                             uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
                             const DecodedInfo* probed, const cudaStream_t* dev_stream, int k) {
@@ -568,64 +624,18 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
   DevImage sdr, map;
   JpegHeader ph, gh;
   const bool want_map = gainmap_out || !sdr_only;  // :1484-1495
-  // both images sizeable: the gain-map JPEG goes to a helper thread with its own stream
-  const bool overlap = want_map && pl >= (256u << 10) && gl >= (256u << 10);
-  struct MapJob {   // lives on this frame until helper_.wait() below
-    JpegRCodec* self;
-    const uint8_t* data;
-    size_t len;
-    DevImage* map;
-    JpegHeader* gh;
-    int dev, k, rc;
-    char err[256];
-  } mj{this, data + go, gl, &map, &gh, 0, k, E_OK, {0}};
-  if (overlap) {
-    if (!ws2_) {
-      ws2_.reset(new Workspace());
-      rc = ws2_->init();
-      if (rc) { ws2_.reset(); return rc; }
-      CUDA_TRY(cudaEventCreateWithFlags(&map_ready_, cudaEventDisableTiming));
-    }
-    ws2_->rewind();
-    CUDA_TRY(cudaGetDevice(&mj.dev));
-    helper_.start([](void* a) {
-      MapJob& j = *static_cast<MapJob*>(a);
-      auto fail_with = [&](int rc, const char* what) { j.rc = rc; snprintf(j.err, sizeof j.err, "%s", what); };
-      if (cudaSetDevice(j.dev) != cudaSuccess) return fail_with(E_ERROR, "cudaSetDevice failed in the gain-map decode thread");
-      j.rc = j.self->decode_jpeg_dev(*j.self->ws2_, j.data, j.len, 2, j.map, j.gh, nullptr, j.k);  // DECODE_STREAM :1486
-      if (j.rc) snprintf(j.err, sizeof j.err, "%s", last_error());
-      else if (cudaEventRecord(j.self->map_ready_, j.self->ws2_->stream()) != cudaSuccess) fail_with(E_ERROR, "cudaEventRecord failed");
-    }, &mj);
-  }
   // into device planes, the colour conversion of an SRGB output writes the caller's plane: it waits for the end
   YccToRgbaParams to_rgba{};
-  rc = decode_jpeg_dev(ws_, data + po, pl, sdr_only ? 1 : 0, &sdr, &ph,
-                       dev_stream && sdr_only ? &to_rgba : nullptr, k);  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS
-  if (overlap) helper_.wait();
+  map_pending_ = false;   // the scratch that held a lazily kept map is being reused
+  rc = decode_pair(data, po, pl, go, gl, sdr_only ? 1 : 0, dev_stream && sdr_only ? &to_rgba : nullptr, want_map, k, &sdr,
+                   &map, &ph, &gh, tr);  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS
   if (rc) return rc;
-  tr.mark("primary jpeg enqueued");
-  ByteView blob = find_marker(data + po, ph, 0xE2, "ICC_PROFILE", 12);
-  sdr.cg = icc_read_gamut(blob.data, blob.size);
-  map_pending_ = false;
   uhdr_gainmap_metadata_t md{};
-  if (want_map) {
-    if (overlap) {
-      if (mj.rc) { set_last_error(mj.err); return mj.rc; }
-      CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), map_ready_, 0));
-      if (kernel_timing_enabled()) ws2_->sync();
-    } else {
-      rc = decode_jpeg_dev(ws_, data + go, gl, 2, &map, &gh, nullptr, k);  // DECODE_STREAM :1486
-      if (rc) return rc;
-    }
-    blob = find_marker(data + go, gh, 0xE2, "ICC_PROFILE", 12);
-    map.cg = icc_read_gamut(blob.data, blob.size);
-    tr.mark("gainmap jpeg enqueued");
-  }
   if (md_out || !sdr_only) {  // :1497-1518
     // the reference reads the gain-map image's markers only when it decodes that image (:1484-1495):
     // metadata alone with SDR output finds no buffer to parse
     if (!want_map) return fail(E_INVALID_PARAM, "received no valid buffer to parse gainmap metadata");
-    blob = find_marker(data + go, gh, 0xE2, "urn:iso:std:iso:ts:21496:-1", 28);
+    const ByteView blob = find_marker(data + go, gh, 0xE2, "urn:iso:std:iso:ts:21496:-1", 28);
     const ByteView xmp = find_marker(data + go, gh, 0xE1, "http://ns.adobe.com/xap/1.0/", 29);
     const ByteView exif = find_marker(data + po, ph, 0xE1, "Exif\0\0", 6);
     rc = parse_gainmap_metadata(blob.data, blob.size, xmp.data, xmp.size, exif.data, exif.size, &md);
@@ -684,6 +694,26 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
   if (rc) return rc;
   rc = ws_.sync();
   tr.mark("pixels on the host");
+  return rc;
+}
+
+int JpegRCodec::decode_images(const uint8_t* data, size_t size, const DecodedInfo& probed, int k, DevImage* sdr,
+                              DevImage* map, uhdr_gainmap_metadata_t* md) {
+  int rc = settle();
+  if (rc) return rc;
+  PhaseTrace tr;
+  ws_.rewind();
+  map_pending_ = false;
+  JpegHeader ph, gh;
+  rc = decode_pair(data, probed.base_off, probed.base_len, probed.gainmap_off, probed.gainmap_len, 0, nullptr, true, k,
+                   sdr, map, &ph, &gh, tr);  // DECODE_TO_YCBCR_CS, DECODE_STREAM
+  if (!rc) {
+    const ByteView iso = find_marker(data + probed.gainmap_off, gh, 0xE2, "urn:iso:std:iso:ts:21496:-1", 28);
+    const ByteView xmp = find_marker(data + probed.gainmap_off, gh, 0xE1, "http://ns.adobe.com/xap/1.0/", 29);
+    const ByteView exif = find_marker(data + probed.base_off, ph, 0xE1, "Exif\0\0", 6);
+    rc = parse_gainmap_metadata(iso.data, iso.size, xmp.data, xmp.size, exif.data, exif.size, md);
+  }
+  if (rc) mark_in_flight();   // as decode(): kernels of both JPEGs may still run
   return rc;
 }
 

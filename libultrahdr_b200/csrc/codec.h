@@ -77,6 +77,12 @@ class JpegRCodec {
   int decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
              uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
              const DecodedInfo* probed = nullptr, const cudaStream_t* dev_stream = nullptr, int k = 1);
+  // The two images decode() hands to applyGainMap, at 1/k: the primary as YCbCr planes (DECODE_TO_YCBCR_CS; Y400,
+  // YUV420 / 422 / 444 at k = 1, Y400 / YUV444 above), the map as Y400 or RGBA8888 (DECODE_STREAM), each with the gamut
+  // of its ICC profile, and the metadata.  `probed`: probe() of the same stream.  Enqueued on ws().stream(); the planes
+  // are this codec's scratch, valid until its next call.
+  int decode_images(const uint8_t* data, size_t size, const DecodedInfo& probed, int k, DevImage* sdr, DevImage* map,
+                    uhdr_gainmap_metadata_t* md);
   // Host wait until what an earlier decode() left in flight is done -- its writes into device planes, or the kernels
   // of a failed call: its scratch (device arenas of both workspaces, the pinned gain tables still waiting for their
   // copy) may be reused after this.
@@ -100,6 +106,11 @@ class JpegRCodec {
   // are returned there, out->v.p[0] stays null
   int decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr,
                       YccToRgbaParams* to_rgba = nullptr, int k = 1);
+  // both JPEGs of a JPEG/R (po / pl, go / gl: their spans in data) on this codec's streams -- the gain map's on the
+  // helper thread when both are sizeable, joined into ws_ -- and the gamuts of their ICC profiles; want_map false: the
+  // primary only.  sdr_mode / to_rgba: decode_jpeg_dev's mode / to_rgba of the primary.
+  int decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go, size_t gl, int sdr_mode, YccToRgbaParams* to_rgba,
+                  bool want_map, int k, DevImage* sdr, DevImage* map, JpegHeader* ph, JpegHeader* gh, PhaseTrace& tr);
   int decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                   uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
                   const DecodedInfo* probed, const cudaStream_t* dev_stream, int k);
@@ -134,6 +145,13 @@ int upload_jpeg_input(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out,
 // uhdr_enc_set_raw_image's checks of one intent's descriptor (ultrahdr_api.cpp:842-1025): its code, the last error
 // set.  The planes are not dereferenced.
 int validate_raw_intent(const uhdr_raw_image_t& img, int intent);
+
+// The *_dev entry points' helpers (capi_stages.cu).  dev_codec: the calling thread's codec for the current device,
+// settled and rewound.  check_dev_planes: a device descriptor's planes present, strides >= widths, elements aligned;
+// check_dev_memory: each plane device memory of the current device.
+int dev_codec(JpegRCodec** out);
+int check_dev_planes(const uhdr_raw_image_t& img, const char* what);
+int check_dev_memory(const uhdr_raw_image_t& img, const char* what);
 
 
 }  // namespace uhdr_b200

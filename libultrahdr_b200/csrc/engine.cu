@@ -330,9 +330,51 @@ void apply_route_stats(unsigned long long out[4]) {
   for (int i = 0; i < 4; i++) out[i] = g_apply_routes[i].load(std::memory_order_relaxed);
 }
 
+bool map_needs_resize(int w, int h, int map_w, int map_h) {  // :1652-1671
+  const float pa = (float)w / h, ga = (float)map_w / map_h;
+  return std::fabs(pa - ga) / pa > 0.01f;
+}
+
+int resize_map_dev(Workspace& ws, const DevImage& map, int w, int h, DevImage* rs) {
+  if (!rs->v.p[0] && alloc_dev_image(ws, map.v.fmt, w, h, 64, rs))
+    return fail(E_UNSUPPORTED, "encountered error while resizing the gainmap image from %ux%u to %ux%u", map.v.w, map.v.h, w, h);
+  ResizeMapParams r;
+  r.src = (const uint8_t*)map.v.p[0];
+  r.src_w = map.v.w; r.src_h = map.v.h; r.src_stride = map.v.stride[0];
+  r.bpp = map.v.fmt == F_RGBA8888 ? 4 : (map.v.fmt == F_RGB888 ? 3 : 1);
+  r.dst = (uint8_t*)rs->v.p[0];
+  r.dst_w = w; r.dst_h = h; r.dst_stride = rs->v.stride[0];
+  TIMED(ws, "resize_gainmap", launch_resize_map(r, ws.stream()));
+  g_apply_routes[3].fetch_add(1, std::memory_order_relaxed);
+  rs->cg = map.cg; rs->ct = map.ct; rs->range = map.range;
+  return E_OK;
+}
+
+static size_t idw_table_floats(int sdr_w, int map_w, int* scale_int, float* scale_f) {
+  const float scale = (float)sdr_w / map_w;
+  const bool integer = scale == std::floor(scale);
+  *scale_int = integer ? (int)(size_t)scale : 0;
+  *scale_f = scale;
+  return integer && *scale_int > 1 ? (size_t)16 * *scale_int * *scale_int : 0;
+}
+
+size_t apply_table_floats(const DevImage& sdr, const DevImage& map) {
+  int si;
+  float sf;
+  return 3 * 1024 + idw_table_floats(sdr.v.w, map.v.w, &si, &sf) + 768 + 4;
+}
+
 int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in,
                       const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                       DevImage* dst) {
+  return apply_gainmap_region(&ws, ws.stream(), ws.luts(), sdr, map_in, md, out_ct, max_display_boost, dst, nullptr,
+                              nullptr, nullptr);
+}
+
+int apply_gainmap_region(Workspace* ws, cudaStream_t stream, const float* luts, const DevImage& sdr,
+                         const DevImage& map_in, const uhdr_gainmap_metadata_t& md, int out_ct,
+                         float max_display_boost, DevImage* dst, const ApplyRegion* region, float* h_tab,
+                         float* d_tab) {
   DevImage map = map_in;
   // validation, jpegr.cpp:1538-1614
   if (!dst || !dst->v.p[0])
@@ -363,31 +405,14 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
     return fail(E_ERROR, "No implementation available for converting from gamut %d to %d", sdr_cg, hdr_cg);
   p.gamut_on_sdr = md.use_base_cg ? 0 : 1;
   p.gamut_identity = ident ? 1 : 0;
-  {  // aspect-ratio check :1652-1671
-    const float pa = (float)sdr.v.w / sdr.v.h, ga = (float)map.v.w / map.v.h;
-    if (std::fabs(pa - ga) / pa > 0.01f) {  // resize_image(gainmap_img, sdr_intent->w, sdr_intent->h)
-      DevImage rs;
-      int rc = alloc_dev_image(ws, map.v.fmt, sdr.v.w, sdr.v.h, 64, &rs);
-      if (rc) return fail(E_UNSUPPORTED, "encountered error while resizing the gainmap image from %ux%u to %ux%u", map.v.w,
-                          map.v.h, sdr.v.w, sdr.v.h);
-      ResizeMapParams r;
-      r.src = (const uint8_t*)map.v.p[0];
-      r.src_w = map.v.w; r.src_h = map.v.h; r.src_stride = map.v.stride[0];
-      r.bpp = map.v.fmt == F_RGBA8888 ? 4 : (map.v.fmt == F_RGB888 ? 3 : 1);
-      r.dst = (uint8_t*)rs.v.p[0];
-      r.dst_w = sdr.v.w; r.dst_h = sdr.v.h; r.dst_stride = rs.v.stride[0];
-      TIMED(ws, "resize_gainmap", launch_resize_map(r, ws.stream()));
-      g_apply_routes[3].fetch_add(1, std::memory_order_relaxed);
-      rs.cg = map.cg; rs.ct = map.ct; rs.range = map.range;
-      map = rs;
-    }
+  if (map_needs_resize(sdr.v.w, sdr.v.h, map.v.w, map.v.h)) {  // resize_image(gainmap_img, sdr_intent->w, sdr_intent->h)
+    if (!ws) return fail(E_ERROR, "the gain map of a region render must have the base image's aspect ratio");
+    DevImage rs;
+    rs.v.p[0] = nullptr;
+    if (int rc = resize_map_dev(*ws, map, sdr.v.w, sdr.v.h, &rs)) return rc;
+    map = rs;
   }
-  const float scale = (float)sdr.v.w / map.v.w;
-  int srnd = (int)std::roundf(scale);
-  if (srnd < 1) srnd = 1;
-  const bool integer = scale == std::floor(scale);
-  p.scale_int = integer ? (int)(size_t)scale : 0;
-  p.scale_f = scale;
+  const size_t idw_floats = idw_table_floats(sdr.v.w, map.v.w, &p.scale_int, &p.scale_f);
   float display_boost = max_display_boost < md.hdr_capacity_max ? max_display_boost : md.hdr_capacity_max;
   float weight;
   if (display_boost != md.hdr_capacity_max) {  // :1680-1689, float log2 (using namespace std)
@@ -401,11 +426,12 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
   GainmapMetadata m;
   static_assert(sizeof(GainmapMetadata) == sizeof(uhdr_gainmap_metadata_t), "layout");
   memcpy(&m, &md, sizeof m);
-  const size_t idw_floats = integer && p.scale_int > 1 ? (size_t)16 * p.scale_int * p.scale_int : 0;
   const size_t tab_floats = 3 * 1024 + idw_floats + 768 + 4;  // + zeroed tile-counter words
-  float* h_tab = (float*)ws.halloc(sizeof(float) * tab_floats);
-  float* d_tab = (float*)ws.dalloc(sizeof(float) * tab_floats);
-  if (!h_tab || !d_tab) return E_MEM;
+  if (!h_tab) {
+    h_tab = (float*)ws->halloc(sizeof(float) * tab_floats);
+    d_tab = (float*)ws->dalloc(sizeof(float) * tab_floats);
+    if (!h_tab || !d_tab) return E_MEM;
+  }
   memset(h_tab + tab_floats - 4, 0, 4 * sizeof(float));
   build_gain_lut(m, weight, h_tab);
   {  // scale-1 shortcut table: gain-map byte -> gain factor.  mapUintToFloat (b / 255.0f), IDW
@@ -422,7 +448,7 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
   if (idw_floats) {
     build_idw_tables(p.scale_int, h_tab + 3 * 1024);   // straight into the pinned staging block
   }
-  CUDA_TRY(cudaMemcpyAsync(d_tab, h_tab, sizeof(float) * tab_floats, cudaMemcpyHostToDevice, ws.stream()));
+  CUDA_TRY(cudaMemcpyAsync(d_tab, h_tab, sizeof(float) * tab_floats, cudaMemcpyHostToDevice, stream));
   p.gain_lut = d_tab;
   p.idw = d_tab + 3 * 1024;
   const bool single = metadata_single_channel(m);
@@ -449,16 +475,21 @@ int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map_in
   p.map_nch = map.v.fmt == F_Y400 ? 1 : 3;
   p.out_ct = out_ct;
   p.out_nits = out_ct == UHDR_CT_HLG ? 1000.0f : 10000.0f;
-  p.luts = ws.luts();
+  p.luts = luts;
   p.dst = (void*)dst->v.p[0];
   p.dst_stride = dst->v.stride[0];
-  if (apply_fast_eligible(p)) {
-    TIMED(ws, "apply_gainmap", launch_apply_fast(p, d_tab + 3 * 1024 + idw_floats, ws.stream()));
-    g_apply_routes[p.scale_int == 1 && out_ct == UHDR_CT_LINEAR ? 0 : 1].fetch_add(1, std::memory_order_relaxed);
-  } else {
-    TIMED(ws, "apply_gainmap", launch_apply_gainmap(p, ws.stream()));
-    g_apply_routes[2].fetch_add(1, std::memory_order_relaxed);
+  if (region) {  // the scale above is the whole image's
+    p.sdr.w = region->w;
+    p.sdr.h = region->h;
+    p.ox = region->ox;
+    p.oy = region->oy;
   }
+  const bool fast = apply_fast_eligible(p);
+  if (ws) ws->t_begin("apply_gainmap");
+  const cudaError_t e = fast ? launch_apply_fast(p, d_tab + 3 * 1024 + idw_floats, stream) : launch_apply_gainmap(p, stream);
+  if (ws) ws->t_end();
+  CUDA_TRY(e);
+  g_apply_routes[!fast ? 2 : p.scale_int == 1 && out_ct == UHDR_CT_LINEAR ? 0 : 1].fetch_add(1, std::memory_order_relaxed);
   return E_OK;
 }
 

@@ -48,6 +48,20 @@ void gainmap_affine_stats(unsigned long long out[2]);
 int apply_gainmap_dev(Workspace& ws, const DevImage& sdr, const DevImage& map,
                       const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                       DevImage* dst /* allocated by caller, fmt F16 / 1010102 */);
+// A rectangle of the image: dst->v.w x dst->v.h pixels starting at (ox, oy), w / h being the same.
+struct ApplyRegion { int ox, oy, w, h; };
+// apply_gainmap_dev on `stream`, with the LUT blob `luts`, of `region` (null: the whole image).  h_tab / d_tab: pinned
+// and device blocks of apply_table_floats(sdr, map) floats for the per-call tables, or null to take them from *ws.  ws
+// null: nothing is timed, and a map whose aspect ratio differs from sdr's is an error (resize it first).
+int apply_gainmap_region(Workspace* ws, cudaStream_t stream, const float* luts, const DevImage& sdr,
+                         const DevImage& map, const uhdr_gainmap_metadata_t& md, int out_ct,
+                         float max_display_boost, DevImage* dst, const ApplyRegion* region, float* h_tab,
+                         float* d_tab);
+size_t apply_table_floats(const DevImage& sdr, const DevImage& map);
+// applyGainMap's aspect-ratio check (jpegr.cpp:1652-1671): the map is resized to w x h first
+bool map_needs_resize(int w, int h, int map_w, int map_h);
+// resize_image of the map to w x h into rs (rs->v.p[0] null: allocated from ws, stride aligned to 64), on ws.stream()
+int resize_map_dev(Workspace& ws, const DevImage& map, int w, int h, DevImage* rs);
 // apply_gainmap_dev launches since process start: [0] k_apply_lin1, [1] k_apply_fast, [2] k_apply_gainmap, [3] k_resize_map
 void apply_route_stats(unsigned long long out[4]);
 int tonemap_dev(Workspace& ws, const DevImage& hdr, DevImage* sdr /* allocated by caller */);

@@ -544,17 +544,20 @@ __device__ __forceinline__ void apply_one(const ApplyParams& p, int x, int y, C3
 }
 
 // one thread = 2 horizontally adjacent pixels (shared chroma sample for 4:2:0 / 4:2:2);
-// a warp writes 512 contiguous bytes of RGBA-F16 (or 256 of 1010102) per row.
+// a warp writes 512 contiguous bytes of RGBA-F16 (or 256 of 1010102) per row.  x, y: relative to the region origin
+// (p.ox, p.oy), which ORG = false takes as 0, 0: the whole-image kernel.
+template <bool ORG>
 __global__ void __launch_bounds__(256) k_apply_gainmap(const ApplyParams p) {
   const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 2;
   const int y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= p.sdr.w || y >= p.sdr.h) return;
   const bool two = x + 1 < p.sdr.w;
-  C3 g0 = fetch_pixel(p.sdr, x, y);
-  C3 g1 = two ? fetch_pixel(p.sdr, x + 1, y) : g0;
+  const int ax = ORG ? p.ox + x : x, ay = ORG ? p.oy + y : y;
+  C3 g0 = fetch_pixel(p.sdr, ax, ay);
+  C3 g1 = two ? fetch_pixel(p.sdr, ax + 1, ay) : g0;
   unsigned o0[2], o1[2] = {0, 0};
-  apply_one(p, x, y, g0, o0);
-  if (two) apply_one(p, x + 1, y, g1, o1);
+  apply_one(p, ax, ay, g0, o0);
+  if (two) apply_one(p, ax + 1, ay, g1, o1);
   if (p.out_ct == CT_LINEAR) {
     uint2* d = (uint2*)p.dst + (size_t)y * p.dst_stride + x;
     if (two && ((((size_t)d) & 15) == 0)) {
@@ -822,11 +825,13 @@ __global__ void __launch_bounds__(128) k_idct_dequant(const IdctPlaneParams p) {
   }
 }
 
-// jdcolor.c ycc_rgb_convert with JCS_EXT_RGBA (alpha 0xFF)
+// jdcolor.c ycc_rgb_convert with JCS_EXT_RGBA (alpha 0xFF).  ORG: a region with an origin other than 0, 0
+template <bool ORG>
 __global__ void __launch_bounds__(256) k_ycc_to_rgba(const YccToRgbaParams p) {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= p.w || y >= p.h) return;
+  const int rx = blockIdx.x * blockDim.x + threadIdx.x;
+  const int ry = blockIdx.y * blockDim.y + threadIdx.y;
+  if (rx >= p.w || ry >= p.h) return;
+  const int x = ORG ? p.ox + rx : rx, y = ORG ? p.oy + ry : ry;   // absolute: every read below
   const size_t i = (size_t)y * p.src_stride + x;
   const int yy = __ldg(p.y + i);
   int xb, xr;
@@ -873,7 +878,7 @@ __global__ void __launch_bounds__(256) k_ycc_to_rgba(const YccToRgbaParams p) {
   const int g = yy + ((-22554 * xb + 32768 - 46802 * xr) >> 16);
   const unsigned px = (unsigned)min(max(r, 0), 255) | ((unsigned)min(max(g, 0), 255) << 8) |
                       ((unsigned)min(max(b, 0), 255) << 16) | 0xFF000000u;
-  ((unsigned*)p.dst)[(size_t)y * p.dst_stride + x] = px;
+  ((unsigned*)p.dst)[(size_t)ry * p.dst_stride + rx] = px;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -915,7 +920,8 @@ cudaError_t launch_gainmap_affine(const AffineParams& p, cudaStream_t s) {
 }
 cudaError_t launch_apply_gainmap(const ApplyParams& p, cudaStream_t s) {
   dim3 b(32, 8);
-  k_apply_gainmap<<<grid2((p.sdr.w + 1) / 2, p.sdr.h, b), b, 0, s>>>(p);
+  if (p.ox | p.oy) k_apply_gainmap<true><<<grid2((p.sdr.w + 1) / 2, p.sdr.h, b), b, 0, s>>>(p);
+  else k_apply_gainmap<false><<<grid2((p.sdr.w + 1) / 2, p.sdr.h, b), b, 0, s>>>(p);
   COUNT_LAUNCH();
   return cudaGetLastError();
 }
@@ -1014,7 +1020,8 @@ cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s) {
 }
 cudaError_t launch_ycc_to_rgba(const YccToRgbaParams& p, cudaStream_t s) {
   dim3 b(32, 8);
-  k_ycc_to_rgba<<<grid2(p.w, p.h, b), b, 0, s>>>(p);
+  if (p.ox | p.oy) k_ycc_to_rgba<true><<<grid2(p.w, p.h, b), b, 0, s>>>(p);
+  else k_ycc_to_rgba<false><<<grid2(p.w, p.h, b), b, 0, s>>>(p);
   COUNT_LAUNCH();
   return cudaGetLastError();
 }

@@ -77,6 +77,10 @@ struct ApplyParams {                // applyGainMap, jpegr.cpp:1533-1831
   void* dst;
   int dst_stride;
   int nan_possible;                 // the gain table is so large that a channel can become inf or NaN
+  // region rendering: sdr.w x sdr.h pixels starting at (ox, oy) of the image whose planes sdr.p / map point to.  Base
+  // reads, chroma indices, map taps and IDW phases use the absolute coordinates, stores are relative to dst; scale_int /
+  // scale_f are those of the whole image.  0, 0 for a whole image.
+  int ox, oy;
 };
 
 struct TonemapParams {              // toneMap, jpegr.cpp:1985-2222
@@ -173,6 +177,9 @@ struct YccToRgbaParams {
   int c_stride, cw, ch;             // chroma plane stride and real (downsampled) size
   uint8_t* dst;                     // RGBA8888
   int dst_stride;                   // pixels
+  // region: w x h pixels starting at (ox, oy) of the planes, stored relative to dst; cw / ch stay the whole image's,
+  // so fancy upsampling reads the real neighbouring chroma
+  int ox, oy;
 };
 
 cudaError_t launch_gainmap_pass1(const GainmapGenParams& p, cudaStream_t s);

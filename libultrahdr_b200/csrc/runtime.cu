@@ -99,7 +99,7 @@ std::vector<ParkedBlock> g_parked[2];              // [0] device memory, [1] pin
 size_t g_parked_bytes[2] = {0, 0};
 constexpr size_t kParkCap[2] = {(size_t)8 << 30, (size_t)4 << 30};
 
-char* take_parked(bool pinned, int device, size_t bytes, size_t* got) {
+char* take_parked(bool pinned, int device, size_t bytes, size_t max_size, size_t* got) {
   std::lock_guard<std::mutex> lk(g_park_mu);
   auto& v = g_parked[pinned ? 1 : 0];
   int best = -1;
@@ -110,7 +110,7 @@ char* take_parked(bool pinned, int device, size_t bytes, size_t* got) {
   // a handle of the same kind asks for the same block sizes in the same order, so near-exact matches
   // are the rule; handing a much larger block to a small request would only force the next large
   // request back to the driver
-  if (best < 0 || v[best].size > bytes + bytes / 4 + ((size_t)1 << 20)) return nullptr;
+  if (best < 0 || v[best].size > max_size) return nullptr;
   char* base = v[best].base;
   *got = v[best].size;
   g_parked_bytes[pinned ? 1 : 0] -= v[best].size;
@@ -170,11 +170,14 @@ void* Arena::alloc(size_t bytes, size_t align) {
       return b.base + off;
     }
   }
-  const size_t min_block = pinned_ ? (size_t)32 << 20 : (size_t)64 << 20;
+  const size_t min_block = min_block_ ? min_block_ : pinned_ ? (size_t)32 << 20 : (size_t)64 << 20;
   size_t sz = bytes > min_block ? bytes : min_block;
   sz = (sz + 4095) / 4096 * 4096;
   if (device_ < 0) cudaGetDevice(&device_);
-  char* base = take_parked(pinned_, device_, sz, &sz);
+  // an exactly sized arena (min_block set: a resident image, kept for long) takes a parked block only if it is
+  // nearly the size asked for
+  const size_t max_size = min_block_ ? sz + sz / 32 : sz + sz / 4 + ((size_t)1 << 20);
+  char* base = take_parked(pinned_, device_, sz, max_size, &sz);
   if (!base) {
     cudaError_t e = pinned_ ? cudaHostAlloc((void**)&base, sz, cudaHostAllocPortable)
                             : cudaMalloc((void**)&base, sz);

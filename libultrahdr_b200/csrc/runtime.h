@@ -70,7 +70,8 @@ size_t trim_parked_blocks();
 
 class Arena {
  public:
-  explicit Arena(bool pinned_host) : pinned_(pinned_host) {}
+  // min_block: the smallest block taken from the driver (0: 64 MiB of device / 32 MiB of pinned memory)
+  explicit Arena(bool pinned_host, size_t min_block = 0) : pinned_(pinned_host), min_block_(min_block) {}
   ~Arena();
   void* alloc(size_t bytes, size_t align = 256);  // nullptr on failure (last error set)
   void rewind();
@@ -84,6 +85,7 @@ class Arena {
   struct Block { char* base; size_t size, used, floor; };
   std::vector<Block> blocks_;
   bool pinned_;
+  size_t min_block_;
   int device_ = -1;  // device the blocks belong to (set at the first allocation)
 };
 

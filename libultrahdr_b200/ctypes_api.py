@@ -85,6 +85,17 @@ def declare_scaled_decode(lib):
     return lib
 
 
+def declare_resident_image(lib):
+    """argument types of the device-resident image entry points (uhdr_b200_image_*, include/uhdr_b200.h)"""
+    lib.uhdr_b200_image_open_dev.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]
+    lib.uhdr_b200_image_info.argtypes = [C.c_void_p] + [C.POINTER(C.c_uint)] * 4 + [C.c_void_p,
+                                                                                     C.POINTER(C.c_size_t)]
+    lib.uhdr_b200_image_render_dev.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_uint, C.c_void_p,
+                                               C.c_void_p]
+    lib.uhdr_b200_image_release.argtypes = [C.c_void_p]
+    return lib
+
+
 def declare_jpeg_encode_stats(lib):
     """uhdr_b200_jpeg_encode_stats(unsigned long long out[10]) on a loaded libuhdr_b200"""
     lib.uhdr_b200_jpeg_encode_stats.argtypes = [C.POINTER(C.c_ulonglong)]
