@@ -749,7 +749,7 @@ static void make_dec_tbl(const uint8_t bits[17], const uint8_t* vals, dec_tbl_t*
     if (bits[l]) {
       t->valoff[l] = p - code;
       for (int i = 0; i < bits[l]; i++, p++, code++) {
-        if (l <= 9) {
+        if (l <= 9 && code < (1 << l)) {  /* a table that is no prefix code (legal while no scan selects it) stays in bounds */
           int lo = code << (9 - l);
           for (int k = 0; k < (1 << (9 - l)); k++) t->look[lo + k] = (uint16_t)((l << 8) | vals[p]);
         }

@@ -24,10 +24,14 @@ typedef struct {
 } jsr_err_t;
 
 static void jsr_error_exit(j_common_ptr cinfo) { longjmp(((jsr_err_t*)cinfo->err)->jb, 1); }
-static void jsr_quiet(j_common_ptr cinfo, int level) { (void)cinfo; (void)level; }
+/* prints nothing, but counts warnings (level -1: corrupt data that libjpeg decodes anyway) like the default does */
+static void jsr_quiet(j_common_ptr cinfo, int level) {
+  if (level < 0) cinfo->err->num_warnings++;
+}
 
 /* info (16 ints): [0] output_width, [1] output_height, [2] num_components, [3] min_DCT_scaled_size, then per
- * component c: [4 + 3c] DCT_scaled_size, [5 + 3c] downsampled_width, [6 + 3c] downsampled_height.
+ * component c < 3: [4 + 3c] DCT_scaled_size, [5 + 3c] downsampled_width, [6 + 3c] downsampled_height; [15] the
+ * warnings libjpeg raised (after a decode; 0 for out == NULL).
  * mode 0: planes back to back, plane c downsampled_width x downsampled_height, tightly packed.
  * mode 1: output_width x output_height RGBA pixels.
  * out == NULL: header and geometry only.  Returns 0, 1 on a libjpeg error, 2 if cap is too small. */
@@ -65,11 +69,13 @@ int jsr_decode(const uint8_t* data, size_t size, int k, int mode, uint8_t* out, 
   info[2] = cinfo.num_components;
   info[3] = cinfo.min_DCT_scaled_size;
   size_t need = 0;
-  for (int c = 0; c < cinfo.num_components && c < 4; c++) {
+  for (int c = 0; c < cinfo.num_components; c++) {
     const jpeg_component_info* ci = &cinfo.comp_info[c];
-    info[4 + 3 * c] = ci->DCT_scaled_size;
-    info[5 + 3 * c] = (int)ci->downsampled_width;
-    info[6 + 3 * c] = (int)ci->downsampled_height;
+    if (c < 3) {
+      info[4 + 3 * c] = ci->DCT_scaled_size;
+      info[5 + 3 * c] = (int)ci->downsampled_width;
+      info[6 + 3 * c] = (int)ci->downsampled_height;
+    }
     need += (size_t)ci->downsampled_width * ci->downsampled_height;
   }
   if (mode == 1) need = (size_t)cinfo.output_width * cinfo.output_height * 4;
@@ -124,6 +130,7 @@ int jsr_decode(const uint8_t* data, size_t size, int k, int mode, uint8_t* out, 
     }
   }
   jpeg_finish_decompress(&cinfo);
+  info[15] = (int)err.pub.num_warnings;
   jpeg_destroy_decompress(&cinfo);
   free(tmp);
   free(rows);

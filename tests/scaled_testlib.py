@@ -20,8 +20,12 @@ SCALES = (1, 2, 4, 8)
 SUBSAMPLING = {"444": 0, "422": 1, "420": 2}
 
 
+def _stale(so, src):
+    return not os.path.exists(so) or os.path.getmtime(so) < os.path.getmtime(os.path.join(ROOT, "oracle", src))
+
+
 def ensure_built():
-    if not os.path.exists(SCALED_ORACLE_SO) or not os.path.exists(SCALED_REF_SO):
+    if _stale(SCALED_ORACLE_SO, "jpeg_scaled_oracle.c") or _stale(SCALED_REF_SO, "jpeg_scaled_ref.c"):
         subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-f", "scaled.mk", "all"],
                               stdout=subprocess.DEVNULL)
 
@@ -43,7 +47,8 @@ def have_harness():
 
 def harness_decode(data, k, mode=0):
     """libjpeg-turbo at scale 1/k.  mode 0 -> (info, [plane c: (downsampled_height, downsampled_width) u8]);
-    mode 1 -> (info, (out_h, out_w, 4) u8 RGBA).  info: [out_w, out_h, ncomp, min_s, then (s, w, h) per component]"""
+    mode 1 -> (info, (out_h, out_w, 4) u8 RGBA).  info: [out_w, out_h, ncomp, min_s, then (s, w, h) per component;
+    [15] the warnings libjpeg-turbo raised]"""
     L = _lib(SCALED_REF_SO)
     buf = (C.c_uint8 * len(data)).from_buffer_copy(data)
     ci = (C.c_int * 16)()
@@ -56,6 +61,7 @@ def harness_decode(data, k, mode=0):
         out = np.zeros(sum(info[5 + 3 * c] * info[6 + 3 * c] for c in range(info[2])), np.uint8)
     rc = L.jsr_decode(buf, C.c_size_t(len(data)), k, mode, out.ctypes.data_as(C.c_void_p), C.c_size_t(out.size), ci)
     assert rc == 0, rc
+    info = list(ci)   # now with [15], the warnings of the decode itself
     if mode == 1:
         return info, out
     planes, o = [], 0
