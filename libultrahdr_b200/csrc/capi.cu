@@ -25,6 +25,7 @@ struct uhdr_codec_private {
   int init_rc = 0;
   int device = -1;  // the CUDA device that was current when the handle was created
   std::string init_err;
+  std::vector<Effect> effects;   // uhdr_add_effect_* in call order; a reset clears it and keeps the capacity
   uhdr_codec_private() {
     if (cudaGetDevice(&device) != cudaSuccess) device = -1;
   }
@@ -81,7 +82,9 @@ struct Encoder : uhdr_codec_private {
   size_t out_cap = 0;
   uhdr_compressed_image_t out_desc{};
   uhdr_error_info_t status = ok();
+  EncodeEffects fx;
   void defaults() {
+    effects.clear();
     raw.clear();
     compressed.clear([](Compressed& c) { c.bytes.clear(); });   // keeps the capacity
     memset(&metadata, 0, sizeof metadata);
@@ -110,7 +113,9 @@ struct Decoder : uhdr_codec_private {
   std::vector<uint8_t> decoded, gainmap;
   uhdr_raw_image_t decoded_desc{}, gainmap_desc{};
   uhdr_error_info_t probe_status = ok(), status = ok();
+  DecodeEffects fx;
   void defaults() {
+    effects.clear();
     stream.clear();
     out_fmt = UHDR_IMG_FMT_64bppRGBAHalfFloat;
     out_ct = UHDR_CT_LINEAR;
@@ -350,11 +355,23 @@ UHDR_API uhdr_error_info_t uhdr_encode(uhdr_codec_private_t* enc) {
   auto sdr = h->raw.find(UHDR_SDR_IMG);
   auto cbase = h->compressed.find(UHDR_BASE_IMG), cgm = h->compressed.find(UHDR_GAIN_MAP_IMG), csdr = h->compressed.find(UHDR_SDR_IMG);
   const bool api4 = cbase != h->compressed.end() && cgm != h->compressed.end();
+  // the effects: refused with a compressed intent, planned on the host for API-0 / API-1 (ultrahdr_api.cpp:1219-1262)
+  const bool fx = !h->effects.empty() && (api4 || hdr != h->raw.end());
+  if (fx && (api4 || csdr != h->compressed.end())) {
+    h->status = err(UHDR_CODEC_INVALID_OPERATION, "image effects are not enabled for inputs with compressed intent");
+    return h->status;
+  }
+  if (fx) {
+    const int rc = h->fx.plan(h->effects, hdr->second.v.w, hdr->second.v.h, hdr->second.v.fmt,
+                              sdr == h->raw.end() ? -1 : sdr->second.v.fmt);
+    if (rc) { h->status = from_rc(rc); return h->status; }
+  }
   if (!api4 && hdr == h->raw.end()) {
     h->status = err(UHDR_CODEC_INVALID_OPERATION, "resources required for uhdr_encode() operation are not present");
     return h->status;
   }
   const size_t cap = api4 ? std::max<size_t>(64 * 1024, 2 * (cbase->second.bytes.size() + cgm->second.bytes.size()))
+                   : fx   ? std::max<size_t>(64 * 1024, (size_t)h->fx.full.w() * h->fx.full.h() * 3 * 2)
                           : std::max<size_t>(64 * 1024, (size_t)hdr->second.v.w * hdr->second.v.h * 3 * 2);  // :1281,:1294
   if (h->out_cap < cap) {
     h->out.reset(new (std::nothrow) uint8_t[cap]);
@@ -381,11 +398,23 @@ UHDR_API uhdr_error_info_t uhdr_encode(uhdr_codec_private_t* enc) {
     h->ensure();
     if (h->init_rc) { h->status = err((uhdr_codec_err_t)h->init_rc, "%s", h->init_err.c_str()); return h->status; }
     h->codec.ws().rewind();
+    // the chain's results go to workspace memory above the floor: the resident inputs stay as they were uploaded
+    DevImage fx_hdr, fx_sdr;
+    const DevImage* hdr_in = &hdr->second;
+    const DevImage* sdr_in = sdr == h->raw.end() ? nullptr : &sdr->second;
+    if (fx) {
+      const GatherPlan* half = h->fx.has_half ? &h->fx.half : nullptr;
+      rc = gather_image(h->codec.ws(), *hdr_in, h->fx.full, half, &fx_hdr);
+      if (!rc && sdr_in) rc = gather_image(h->codec.ws(), *sdr_in, h->fx.full, half, &fx_sdr);
+      if (rc) { h->status = from_rc(rc); return h->status; }
+      hdr_in = &fx_hdr;
+      if (sdr_in) sdr_in = &fx_sdr;
+    }
     if (csdr != h->compressed.end())  // API-2 (raw sdr intent given too) / API-3
       rc = h->codec.encode_with_compressed_sdr(hdr->second, sdr == h->raw.end() ? nullptr : &sdr->second, csdr->second.bytes.data(),
                                                csdr->second.bytes.size(), csdr->second.cg, cfg, h->out.get(), cap, &n);
     else
-      rc = h->codec.encode(hdr->second, sdr == h->raw.end() ? nullptr : &sdr->second, cfg, h->quality[UHDR_BASE_IMG],
+      rc = h->codec.encode(*hdr_in, sdr_in, cfg, h->quality[UHDR_BASE_IMG],
                            h->exif.empty() ? nullptr : h->exif.data(), h->exif.size(), h->out.get(), cap, &n);
   }
   h->status = from_rc(rc);
@@ -527,8 +556,10 @@ UHDR_API uhdr_error_info_t uhdr_decode(uhdr_codec_private_t* dec) {
   h->gainmap_desc.planes[0] = nullptr;
   h->gainmap_desc.stride[0] = h->info.gm_width;
   h->codec.set_lazy_gainmap(true);  // the map leaves HBM only if uhdr_get_decoded_gainmap_image() is called
+  if (!h->effects.empty()) h->fx.plan(h->effects, w, ht, h->info.gm_width, h->info.gm_height);
   int rc = h->codec.decode(h->stream.data(), h->stream.size(), h->out_ct, h->out_fmt, h->max_boost, &h->decoded_desc,
-                           &h->gainmap_desc, nullptr, &h->info);   // uhdr_dec_probe above already located the two images
+                           &h->gainmap_desc, nullptr, &h->info,   // uhdr_dec_probe above already located the two images
+                           nullptr, 1, h->effects.empty() ? nullptr : &h->fx);
   h->status = from_rc(rc);
   return h->status;
 }
@@ -556,14 +587,32 @@ UHDR_API uhdr_error_info_t uhdr_enable_gpu_acceleration(uhdr_codec_private_t* co
   if (!codec) return err(UHDR_CODEC_INVALID_PARAM, "received nullptr for uhdr codec instance");
   return ok();  // the CUDA path is the only path
 }
-static uhdr_error_info_t no_effects(uhdr_codec_private_t* codec) {
+// ultrahdr_api.cpp:2113-2230: null handle, bad argument, then sailed (a decoder takes effects after uhdr_dec_probe).
+// Crop and resize take any values here; uhdr_encode / uhdr_decode check them against the images.
+static uhdr_error_info_t add_effect(uhdr_codec_private_t* codec, const Effect& e, const char* bad_arg) {
   if (!codec) return err(UHDR_CODEC_INVALID_PARAM, "received nullptr for uhdr codec instance");
-  return err(UHDR_CODEC_UNSUPPORTED_FEATURE, "image effects (editorhelper.cpp) are outside the CUDA hot path");
+  if (bad_arg) return err(UHDR_CODEC_INVALID_PARAM, "%s", bad_arg);
+  if (codec->sailed)
+    return err(UHDR_CODEC_INVALID_OPERATION, "An earlier call to uhdr_encode()/uhdr_decode() has switched the context "
+               "from configurable state to end state. The context is no longer configurable. To reuse, call reset()");
+  codec->effects.push_back(e);
+  return ok();
 }
-UHDR_API uhdr_error_info_t uhdr_add_effect_mirror(uhdr_codec_private_t* c, uhdr_mirror_direction_t) { return no_effects(c); }
-UHDR_API uhdr_error_info_t uhdr_add_effect_rotate(uhdr_codec_private_t* c, int) { return no_effects(c); }
-UHDR_API uhdr_error_info_t uhdr_add_effect_crop(uhdr_codec_private_t* c, int, int, int, int) { return no_effects(c); }
-UHDR_API uhdr_error_info_t uhdr_add_effect_resize(uhdr_codec_private_t* c, int, int) { return no_effects(c); }
+UHDR_API uhdr_error_info_t uhdr_add_effect_mirror(uhdr_codec_private_t* c, uhdr_mirror_direction_t direction) {
+  const bool bad = direction != UHDR_MIRROR_HORIZONTAL && direction != UHDR_MIRROR_VERTICAL;
+  return add_effect(c, {FX_MIRROR, direction, 0, 0, 0},
+                    bad ? "unsupported direction, expects one of {UHDR_MIRROR_HORIZONTAL, UHDR_MIRROR_VERTICAL}" : nullptr);
+}
+UHDR_API uhdr_error_info_t uhdr_add_effect_rotate(uhdr_codec_private_t* c, int degrees) {
+  const bool bad = degrees != 90 && degrees != 180 && degrees != 270;
+  return add_effect(c, {FX_ROTATE, degrees, 0, 0, 0}, bad ? "unsupported degrees, expects one of {90, 180, 270}" : nullptr);
+}
+UHDR_API uhdr_error_info_t uhdr_add_effect_crop(uhdr_codec_private_t* c, int left, int right, int top, int bottom) {
+  return add_effect(c, {FX_CROP, left, right, top, bottom}, nullptr);
+}
+UHDR_API uhdr_error_info_t uhdr_add_effect_resize(uhdr_codec_private_t* c, int width, int height) {
+  return add_effect(c, {FX_RESIZE, width, height, 0, 0}, nullptr);
+}
 
 // ---- measurement hooks (include/uhdr_b200.h) -------------------------------------------------------
 UHDR_API void uhdr_b200_set_kernel_timing(int on) { set_kernel_timing(on != 0); }

@@ -540,10 +540,11 @@ int JpegRCodec::probe(const uint8_t* data, size_t size, DecodedInfo* info) {
 
 int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                        uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                       const DecodedInfo* probed, const cudaStream_t* dev_stream, int k) {
+                       const DecodedInfo* probed, const cudaStream_t* dev_stream, int k, const DecodeEffects* fx) {
   int rc = settle();
   if (rc) return rc;
-  rc = decode_body(data, size, out_ct, out_fmt, max_display_boost, dest, gainmap_out, md_out, probed, dev_stream, k);
+  if (fx && (dev_stream || k != 1)) return fail(E_UNSUPPORTED, "image effects apply to host outputs at full size only");
+  rc = decode_body(data, size, out_ct, out_fmt, max_display_boost, dest, gainmap_out, md_out, probed, dev_stream, k, fx);
   // an error can leave kernels of both JPEGs in flight on this codec's streams; the next call on it may run on a
   // caller's stream that is not ordered against them, so settle() has to wait for them before the scratch is reused
   if (rc) mark_in_flight();
@@ -607,7 +608,8 @@ int JpegRCodec::decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go
 
 int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                             uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                            const DecodedInfo* probed, const cudaStream_t* dev_stream, int k) {
+                            const DecodedInfo* probed, const cudaStream_t* dev_stream, int k,
+                            const DecodeEffects* fx) {
   (void)out_fmt;
   PhaseTrace tr;
   int rc = E_OK;
@@ -647,24 +649,27 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
     tr.mark("writes enqueued");
     return rc;
   }
-  if (gainmap_out) {
-    gainmap_out->fmt = (uhdr_img_fmt_t)map.v.fmt;
-    gainmap_out->w = map.v.w;
-    gainmap_out->h = map.v.h;
+  // the effects' map: gathered here, from the map apply reads (the gather does not change its source)
+  DevImage omap = map;
+  if (fx && !fx->rc && gainmap_out && (rc = gather_image(ws_, map, fx->map, nullptr, &omap))) return rc;
+  if (gainmap_out && !(fx && fx->rc)) {
+    gainmap_out->fmt = (uhdr_img_fmt_t)omap.v.fmt;
+    gainmap_out->w = omap.v.w;
+    gainmap_out->h = omap.v.h;
     gainmap_out->cg = UHDR_CG_UNSPECIFIED;
     gainmap_out->ct = UHDR_CT_UNSPECIFIED;
     gainmap_out->range = UHDR_CR_FULL_RANGE;
     if (!gainmap_out->planes[0] && lazy_gainmap_) {
-      gainmap_out->stride[0] = map.v.w;
-      last_map_ = map;
+      gainmap_out->stride[0] = omap.v.w;
+      last_map_ = omap;
       map_pending_ = true;
     } else {
       if (!gainmap_out->planes[0]) {  // handle-owned result: pinned memory of this codec, valid until its next decode
-        gainmap_out->stride[0] = map.v.w;
-        gainmap_out->planes[0] = ws_.halloc((size_t)map.v.w * map.v.h * (map.v.fmt == F_Y400 ? 1 : 4));
+        gainmap_out->stride[0] = omap.v.w;
+        gainmap_out->planes[0] = ws_.halloc((size_t)omap.v.w * omap.v.h * (omap.v.fmt == F_Y400 ? 1 : 4));
         if (!gainmap_out->planes[0]) return E_MEM;
       }
-      rc = download_image(ws_, map, gainmap_out);
+      rc = download_image(ws_, omap, gainmap_out);
       if (rc) return rc;
     }
   }
@@ -683,10 +688,19 @@ int JpegRCodec::decode_body(const uint8_t* data, size_t size, int out_ct, int ou
     dest->cg = (uhdr_color_gamut_t)dst.cg;
     dest->ct = (uhdr_color_transfer_t)out_ct;
   }
+  if (fx) {   // ultrahdr_api.cpp:1996-1998: the effects follow a successful decodeJPEGR
+    if (fx->rc) return fail(fx->rc, "%s", fx->detail);
+    DevImage out;
+    rc = gather_image(ws_, dst, fx->image, nullptr, &out);
+    if (rc) return rc;
+    dst = out;
+    dest->w = dst.v.w;
+    dest->h = dst.v.h;
+  }
   dest->range = UHDR_CR_FULL_RANGE;
   if (!dest->planes[0]) {  // handle-owned result (see above)
-    dest->stride[0] = sdr.v.w;
-    dest->planes[0] = ws_.halloc((size_t)sdr.v.w * sdr.v.h * (dest->fmt == UHDR_IMG_FMT_64bppRGBAHalfFloat ? 8 : 4));
+    dest->stride[0] = dst.v.w;
+    dest->planes[0] = ws_.halloc((size_t)dst.v.w * dst.v.h * (dest->fmt == UHDR_IMG_FMT_64bppRGBAHalfFloat ? 8 : 4));
     if (!dest->planes[0]) return E_MEM;
   }
   tr.mark("apply enqueued");

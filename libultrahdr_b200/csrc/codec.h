@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "container.h"
+#include "effects.h"
 #include "engine.h"
 #include "jpeg.h"
 
@@ -74,9 +75,13 @@ class JpegRCodec {
   // two planes are ordered after the work enqueued earlier on *dev_stream, and *dev_stream waits for them.  The
   // call returns without waiting for either; settle() (run by the next decode()) waits for the writes.
   // `k` (1, 2, 4, 8): both JPEGs are decoded at 1/k size (jpeg_scaled_geometry) and the gain map is applied to those.
+  // `fx` (host outputs at k = 1 only): the editor chain planned for this file's sizes; the output image and the map
+  // are gathered through it in HBM, and dest / gainmap_out get the sizes it ends with.  A planned error is returned
+  // once everything before it has succeeded, as the reference applies effects after decodeJPEGR.
   int decode(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
              uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-             const DecodedInfo* probed = nullptr, const cudaStream_t* dev_stream = nullptr, int k = 1);
+             const DecodedInfo* probed = nullptr, const cudaStream_t* dev_stream = nullptr, int k = 1,
+             const DecodeEffects* fx = nullptr);
   // The two images decode() hands to applyGainMap, at 1/k: the primary as YCbCr planes (DECODE_TO_YCBCR_CS; Y400,
   // YUV420 / 422 / 444 at k = 1, Y400 / YUV444 above), the map as Y400 or RGBA8888 (DECODE_STREAM), each with the gamut
   // of its ICC profile, and the metadata.  `probed`: probe() of the same stream.  Enqueued on ws().stream(); the planes
@@ -113,7 +118,7 @@ class JpegRCodec {
                   bool want_map, int k, DevImage* sdr, DevImage* map, JpegHeader* ph, JpegHeader* gh, PhaseTrace& tr);
   int decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                   uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
-                  const DecodedInfo* probed, const cudaStream_t* dev_stream, int k);
+                  const DecodedInfo* probed, const cudaStream_t* dev_stream, int k, const DecodeEffects* fx);
   // record where this codec's streams are (both joined into ws_); settle() waits for that point
   int mark_in_flight();
   int write_dev_outputs(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
