@@ -140,6 +140,33 @@ UHDR_EXTERN int uhdr_b200_scaled_dims(const void* data, size_t size, int k, unsi
 UHDR_EXTERN int uhdr_b200_decode_scaled_dev(const void* data, size_t size, int k, int out_ct, float max_display_boost,
                                             uhdr_raw_image_t* dest_dev, uhdr_raw_image_t* gainmap_dev,
                                             uhdr_gainmap_metadata_t* metadata_out, void* stream);
+/* Batched decoding: uhdr_b200_decode_scaled_dev of n files in one call, with one entropy-decoding pass and one inverse
+ * DCT per reduced size over both JPEGs of every file, then each file's colour conversion and gain-map application.
+ * For many small outputs (thumbnails, previews) this saves the fixed launches and host waits a single decode costs.
+ *  - Same bytes: each item's dest_dev, gainmap_dev and metadata_out get byte for byte what uhdr_b200_decode_scaled_dev
+ *    writes for that file with the same k, out_ct and max_display_boost.  dest_dev->fmt is read per item (each must
+ *    pair with out_ct), so one batch may mix formats; the sizes are those uhdr_b200_scaled_dims gives.
+ *  - Errors per item: status is the code the single call returns for that file (corrupt data, no metadata, 4:2:2 at
+ *    k > 1, a bad descriptor).  A failing item gets nothing written into its buffers; the others are unaffected.  The
+ *    return value is UHDR_CODEC_OK when every item succeeded, else the first failing item's code, and
+ *    uhdr_b200_last_error() names that item's index and gives its message.  An error of the whole call (CUDA, device
+ *    memory) is returned and set as the status of every item without an error of its own.
+ *  - n < 1, a k outside {1, 2, 4, 8} or a null items give UHDR_CODEC_INVALID_PARAM and decode nothing.
+ *  - Stream order, host blocking and threads: uhdr_b200_decode_dev's rules.  The writes are ordered after the work
+ *    enqueued earlier on `stream`, later work on it sees them, the call may return before they land, and the next
+ *    call on the thread first waits for them.  State is per host thread and device.
+ *  - A batch whose scratch would exceed a device-memory budget (4 GiB; the environment variable
+ *    UHDR_B200_BATCH_GROUP_BYTES sets another) is decoded in groups, one after the other, with the same results. */
+typedef struct uhdr_b200_decode_item {
+  const void* data;                      /* one JPEG/R file, host memory */
+  size_t size;
+  uhdr_raw_image_t* dest_dev;            /* as uhdr_b200_decode_scaled_dev's dest_dev */
+  uhdr_raw_image_t* gainmap_dev;         /* optional, as there */
+  uhdr_gainmap_metadata_t* metadata_out; /* optional, as there */
+  int status;                            /* out: this item's uhdr_codec_err_t */
+} uhdr_b200_decode_item_t;
+UHDR_EXTERN int uhdr_b200_decode_batch_dev(uhdr_b200_decode_item_t* items, int n, int k, int out_ct, float max_display_boost,
+                                           void* stream);
 /* uhdr_b200_jpeg_decode of one JPEG at 1/k (stage hook, host buffers).  k = 1 is uhdr_b200_jpeg_decode.  For k > 1,
  * mode 0 gives Y400 or YUV444 planes of ceil(w / k) x ceil(h / k) samples, back to back at stride = width; mode 1
  * gives RGBA8888 at that size. */

@@ -387,15 +387,16 @@ int check_out(const void* out, size_t* out_size) {
 }
 }  // namespace
 
-// uhdr_b200_decode_dev (k = 1) and uhdr_b200_decode_scaled_dev: sizes checked against the 1/k ones
-static int decode_dev(const void* data, size_t size, int k, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
-                      uhdr_raw_image_t* gainmap, uhdr_gainmap_metadata_t* metadata_out, void* stream) {
+// the checks of uhdr_b200_decode_dev (k = 1) and uhdr_b200_decode_scaled_dev that need no device, sizes against the 1/k
+// ones; *info: the probed file at 1/k
+static int check_decode_args(const void* data, size_t size, int k, int out_ct, float max_display_boost, const uhdr_raw_image_t* dest,
+                             const uhdr_raw_image_t* gainmap, DecodedInfo* out) {
   // uhdr_dec_set_image, uhdr_dec_set_out_max_display_boost and uhdr_decode's checks, in their order
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed img->data field");
   if (!dest) return fail(E_INVALID_PARAM, "received nullptr for destination image");
   if (!std::isfinite(max_display_boost) || max_display_boost < 1.0f)
     return fail(E_INVALID_PARAM, "invalid display boost %f, expects to be >= 1.0f}", max_display_boost);
-  DecodedInfo info;
+  DecodedInfo& info = *out;
   int rc = JpegRCodec().probe((const uint8_t*)data, size, &info);  // host only
   if (rc) return rc;
   scale_dims(&info, k);
@@ -415,16 +416,31 @@ static int decode_dev(const void* data, size_t size, int k, int out_ct, float ma
     if (!gainmap->planes[0] || gainmap->stride[0] < gainmap->w)
       return fail(E_INVALID_PARAM, "gain-map image: null plane or stride %u < width %u", gainmap->stride[0], gainmap->w);
   }
-  JpegRCodec* c = nullptr;
-  if ((rc = dev_codec(&c))) return rc;
-  if ((rc = check_dev_memory(*dest, "destination"))) return rc;
+  return E_OK;
+}
+
+// ... and those that need the device, after dev_codec()
+static int check_decode_memory(const uhdr_raw_image_t* dest, const uhdr_raw_image_t* gainmap, const DecodedInfo& info) {
+  int rc = check_dev_memory(*dest, "destination");
+  if (rc) return rc;
   if (gainmap) {
     uhdr_raw_image_t g = *gainmap;
     g.fmt = info.gm_channels == 1 ? UHDR_IMG_FMT_8bppYCbCr400 : UHDR_IMG_FMT_32bppRGBA8888;  // what the call writes
     if ((rc = check_dev_planes(g, "gain-map image")) || (rc = check_dev_memory(g, "gain-map image"))) return rc;
   }
+  return E_OK;
+}
+
+static int decode_dev(const void* data, size_t size, int k, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
+                      uhdr_raw_image_t* gainmap, uhdr_gainmap_metadata_t* metadata_out, void* stream) {
+  DecodedInfo info;
+  int rc = check_decode_args(data, size, k, out_ct, max_display_boost, dest, gainmap, &info);
+  if (rc) return rc;
+  JpegRCodec* c = nullptr;
+  if ((rc = dev_codec(&c))) return rc;
+  if ((rc = check_decode_memory(dest, gainmap, info))) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
-  return c->decode((const uint8_t*)data, size, out_ct, fmt, max_display_boost, dest, gainmap, metadata_out, &info, &st, k);
+  return c->decode((const uint8_t*)data, size, out_ct, dest->fmt, max_display_boost, dest, gainmap, metadata_out, &info, &st, k);
 }
 
 UHDR_API int uhdr_b200_decode_dev(const void* data, size_t size, int out_ct, float max_display_boost, uhdr_raw_image_t* dest,
@@ -437,6 +453,50 @@ UHDR_API int uhdr_b200_decode_scaled_dev(const void* data, size_t size, int k, i
                                          uhdr_gainmap_metadata_t* metadata_out, void* stream) {
   if (!valid_scale(k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
   return decode_dev(data, size, k, out_ct, max_display_boost, dest, gainmap, metadata_out, stream);
+}
+
+UHDR_API int uhdr_b200_decode_batch_dev(uhdr_b200_decode_item_t* items, int n, int k, int out_ct, float max_display_boost,
+                                        void* stream) {
+  if (!items) return fail(E_INVALID_PARAM, "received nullptr for the items");
+  if (n < 1) return fail(E_INVALID_PARAM, "received %d items, expects at least 1", n);
+  if (!valid_scale(k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
+  static thread_local std::vector<DecodeBatchItem> its;  // grow-only: a batch of the same or a smaller size takes no heap
+  if ((int)its.size() < n) its.resize(n);
+  for (int i = 0; i < n; i++) {
+    const uhdr_b200_decode_item_t& in = items[i];
+    DecodeBatchItem& b = its[i];
+    b.data = (const uint8_t*)in.data;
+    b.size = in.size;
+    b.dest = in.dest_dev;
+    b.gainmap = in.gainmap_dev;
+    b.md_out = in.metadata_out;
+    b.rc = check_decode_args(in.data, in.size, k, out_ct, max_display_boost, in.dest_dev, in.gainmap_dev, &b.info);
+    if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
+  }
+  JpegRCodec* c = nullptr;
+  int rc = dev_codec(&c);
+  for (int i = 0; i < n && !rc; i++) {
+    DecodeBatchItem& b = its[i];
+    if (!b.rc && (b.rc = check_decode_memory(b.dest, b.gainmap, b.info))) snprintf(b.err, sizeof b.err, "%s", last_error());
+  }
+  if (!rc) {
+    size_t group = size_t(4) << 30;
+    if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
+    rc = c->decode_batch(its.data(), n, k, out_ct, max_display_boost, (cudaStream_t)stream, group);
+  }
+  std::string call_err = rc ? last_error() : "";
+  int first = -1;
+  for (int i = 0; i < n; i++) {
+    DecodeBatchItem& b = its[i];
+    if (rc && !b.rc) {  // an error of the whole call: every item without its own
+      b.rc = rc;
+      snprintf(b.err, sizeof b.err, "%s", call_err.c_str());
+    }
+    items[i].status = b.rc;
+    if (b.rc && first < 0) first = i;
+  }
+  if (first < 0) return E_OK;
+  return fail(its[first].rc, "item %d: %s", first, its[first].err);
 }
 
 UHDR_API int uhdr_b200_scaled_dims(const void* data, size_t size, int k, unsigned* w, unsigned* h, unsigned* gm_w,

@@ -401,8 +401,9 @@ JpegRCodec::~JpegRCodec() {
   if (writes_done_) cudaEventDestroy(writes_done_);
 }
 
-int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* h,
-                                YccToRgbaParams* to_rgba, int k) {
+// decode_jpeg_dev up to the entropy decoding: the header, its checks, the output planes
+static int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, int mode, int k, DevImage* out, JpegHeader* h,
+                             JpegDecodeJob* j) {
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed image data");
   if (size == 0) return fail(E_INVALID_PARAM, "received bad compressed image size %zd", size);
   int rc = jpeg_read_header(data, size, h);
@@ -417,7 +418,7 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
   // reduced size (k > 1): every component must come out of the IDCT at the output size; other samplings would
   // need libjpeg's upsampler at the reduced size
   const bool scaled = k != 1;
-  JpegScaled g;
+  JpegScaled& g = j->g;
   if (scaled) {
     if ((rc = jpeg_scaled_geometry(f, k, &g))) return rc;
     if (!g.full_chroma())
@@ -429,8 +430,8 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
   out->v.full_range = 1;
   out->v.w = scaled ? g.width : f.width;
   out->v.h = scaled ? g.height : f.height;
-  uint8_t* planes[3] = {nullptr, nullptr, nullptr};
-  int strides[3] = {0, 0, 0};
+  uint8_t** planes = j->planes;
+  int* strides = j->strides;
   // scaled planes share one stride: the 4:4:4 colour conversion and the apply kernels index chroma with luma's
   int common = 0;
   for (int c = 0; scaled && c < f.ncomp; c++) common = std::max(common, f.comp[c].wblocks * g.s[c]);
@@ -439,30 +440,19 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     planes[c] = (uint8_t*)ws.dalloc((size_t)strides[c] * f.comp[c].hblocks * (scaled ? g.s[c] : 8));
     if (!planes[c]) return E_MEM;
   }
-  // entropy decoding: on the device (huffdec.cu).  The host decoder is not a size-based alternative: it runs only
-  // for streams the parallel decoder declines (restart markers, no fixed point, inconsistent data -- it also
-  // produces the reference's error texts for those) or when a test / triage session selects it (mode 1).
-  const int dec_mode = jpeg_get_entropy_decoder();
-  bool on_device = dec_mode != 1;
-  if (on_device) {
-    int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
-    rc = jpeg_entropy_decode_dev(ws, data, size, *h, d_coefs);
-    if (rc == kHuffDecFallback) on_device = false;
-    else if (rc) return rc;
-    else rc = scaled ? jpeg_idct_scaled_dev(ws, *h, g, d_coefs, planes, strides) : jpeg_idct_dev(ws, *h, d_coefs, planes, strides);
-    if (on_device && rc) return rc;
-  }
-  if (!on_device) {
-    int16_t* h_coefs[3] = {nullptr, nullptr, nullptr};
-    for (int c = 0; c < f.ncomp; c++) {
-      h_coefs[c] = (int16_t*)ws.halloc(f.blocks(c) * 128);
-      if (!h_coefs[c]) return E_MEM;
-    }
-    rc = jpeg_host_decode_coefs(data, size, *h, h_coefs);
-    if (rc) return rc;
-    rc = scaled ? jpeg_inverse_scaled_dev(ws, *h, g, h_coefs, planes, strides) : jpeg_inverse_dev(ws, *h, h_coefs, planes, strides);
-    if (rc) return rc;
-  }
+  j->mode = mode;
+  j->k = k;
+  return E_OK;
+}
+
+// decode_jpeg_dev after the inverse DCT: the colour conversion (mode 1) or the planes' format (mode 0)
+static int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, DevImage* out, YccToRgbaParams* to_rgba) {
+  const JpegFrame& f = h->frame;
+  const int mode = j.mode;
+  const bool scaled = j.k != 1;
+  uint8_t* const* planes = j.planes;
+  const int* strides = j.strides;
+  int rc = E_OK;
   if (mode == 1) {
     const bool s444 = f.max_h == 1 && f.max_v == 1, s422 = f.max_h == 2 && f.max_v == 1, s420 = f.max_h == 2 && f.max_v == 2;
     if (!scaled && (!(s444 || s422 || s420) || f.comp[0].h_samp != f.max_h || f.comp[0].v_samp != f.max_v || f.comp[1].h_samp != 1 ||
@@ -506,6 +496,43 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     out->v.stride[c] = strides[c];
   }
   return E_OK;
+}
+
+int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* h,
+                                YccToRgbaParams* to_rgba, int k) {
+  JpegDecodeJob j;
+  int rc = decode_jpeg_begin(ws, data, size, mode, k, out, h, &j);
+  if (rc) return rc;
+  const JpegFrame& f = h->frame;
+  const bool scaled = k != 1;
+  const JpegScaled& g = j.g;
+  uint8_t** planes = j.planes;
+  int* strides = j.strides;
+  // entropy decoding: on the device (huffdec.cu).  The host decoder is not a size-based alternative: it runs only
+  // for streams the parallel decoder declines (restart markers, no fixed point, inconsistent data -- it also
+  // produces the reference's error texts for those) or when a test / triage session selects it (mode 1).
+  const int dec_mode = jpeg_get_entropy_decoder();
+  bool on_device = dec_mode != 1;
+  if (on_device) {
+    int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
+    rc = jpeg_entropy_decode_dev(ws, data, size, *h, d_coefs);
+    if (rc == kHuffDecFallback) on_device = false;
+    else if (rc) return rc;
+    else rc = scaled ? jpeg_idct_scaled_dev(ws, *h, g, d_coefs, planes, strides) : jpeg_idct_dev(ws, *h, d_coefs, planes, strides);
+    if (on_device && rc) return rc;
+  }
+  if (!on_device) {
+    int16_t* h_coefs[3] = {nullptr, nullptr, nullptr};
+    for (int c = 0; c < f.ncomp; c++) {
+      h_coefs[c] = (int16_t*)ws.halloc(f.blocks(c) * 128);
+      if (!h_coefs[c]) return E_MEM;
+    }
+    rc = jpeg_host_decode_coefs(data, size, *h, h_coefs);
+    if (rc) return rc;
+    rc = scaled ? jpeg_inverse_scaled_dev(ws, *h, g, h_coefs, planes, strides) : jpeg_inverse_dev(ws, *h, h_coefs, planes, strides);
+    if (rc) return rc;
+  }
+  return decode_jpeg_end(ws, h, j, out, to_rgba);
 }
 
 int JpegRCodec::probe(const uint8_t* data, size_t size, DecodedInfo* info) {
@@ -754,18 +781,40 @@ int JpegRCodec::mark_in_flight() {
 int JpegRCodec::write_dev_outputs(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
                                   const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                                   uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, cudaStream_t caller) {
+  if (int rc = check_dev_outputs(sdr, map, out_ct, dest, gainmap_out)) return rc;
+  if (int rc = join_caller(caller)) return rc;
+  if (int rc = enqueue_dev_writes(sdr, map, to_rgba, md, out_ct, max_display_boost, dest, gainmap_out)) return rc;
+  // this codec's stream waits for the caller's: settle() keeps the next call off the scratch read above
+  if (int rc = mark_in_flight()) return rc;
+  CUDA_TRY(cudaStreamWaitEvent(caller, writes_done_, 0));
+  return E_OK;
+}
+
+int JpegRCodec::check_dev_outputs(const DevImage& sdr, const DevImage& map, int out_ct, const uhdr_raw_image_t* dest,
+                                  const uhdr_raw_image_t* gainmap_out) {
   const bool sdr_only = out_ct == UHDR_CT_SRGB;
   if ((int)dest->w != sdr.v.w || (int)dest->h != sdr.v.h)
     return fail(E_INVALID_PARAM, "destination image is %ux%u, the decoded image %dx%d", dest->w, dest->h, sdr.v.w, sdr.v.h);
   if (sdr_only && dest->fmt != UHDR_IMG_FMT_32bppRGBA8888)
     return fail(E_INVALID_PARAM, "unsupported output pixel format and output color transfer pair");
-  const int map_esz = map.v.fmt == F_Y400 ? 1 : 4;
   if (gainmap_out && ((int)gainmap_out->w != map.v.w || (int)gainmap_out->h != map.v.h))
     return fail(E_INVALID_PARAM, "gain-map image is %ux%u, the decoded gain map %dx%d", gainmap_out->w, gainmap_out->h,
                 map.v.w, map.v.h);
+  return E_OK;
+}
+
+int JpegRCodec::join_caller(cudaStream_t caller) {
   if (!caller_ready_) CUDA_TRY(cudaEventCreateWithFlags(&caller_ready_, cudaEventDisableTiming));
   CUDA_TRY(cudaEventRecord(caller_ready_, caller));
   CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), caller_ready_, 0));
+  return E_OK;
+}
+
+int JpegRCodec::enqueue_dev_writes(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
+                                   const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
+                                   uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out) {
+  const bool sdr_only = out_ct == UHDR_CT_SRGB;
+  const int map_esz = map.v.fmt == F_Y400 ? 1 : 4;
   if (sdr_only) {
     YccToRgbaParams p = to_rgba;
     p.dst = (uint8_t*)dest->planes[0];
@@ -797,9 +846,148 @@ int JpegRCodec::write_dev_outputs(const DevImage& sdr, const DevImage& map, cons
                                (size_t)map.v.stride[0] * map_esz, (size_t)map.v.w * map_esz, map.v.h,
                                cudaMemcpyDeviceToDevice, ws_.stream()));
   }
-  // this codec's stream waits for the caller's: settle() keeps the next call off the scratch read above
-  if (int rc = mark_in_flight()) return rc;
+  return E_OK;
+}
+
+static void batch_item_fail(DecodeBatchItem& it, int rc, const char* msg) {
+  it.rc = rc;
+  snprintf(it.err, sizeof it.err, "%s", msg);
+}
+
+int JpegRCodec::decode_batch(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller,
+                             size_t group_bytes) {
+  int rc = E_OK;
+  for (int g0 = 0; g0 < n && !rc;) {
+    // a group: as many items as fit the scratch budget (at least one); the entropy-coded bytes of a group stay below
+    // 2^29 so that every bit position of the group fits 32 bits
+    size_t bytes = 0, coded = 0;
+    int g1 = g0;
+    for (; g1 < n; g1++) {
+      const DecodedInfo& in = items[g1].info;
+      // coefficients (128 B per 8x8 block, at most 3 components at full size) and their DC terms, planes, coded bits
+      const size_t px = (size_t)in.width * k * in.height * k + (size_t)in.gm_width * k * in.gm_height * k;
+      const size_t b = px * 7 + (size_t)(in.width * in.height + in.gm_width * in.gm_height) * 16 + 2 * items[g1].size;
+      if (g1 > g0 && (bytes + b > group_bytes || coded + items[g1].size >= (1u << 29))) break;
+      bytes += b;
+      coded += items[g1].size;
+    }
+    if (g0 > 0 && (rc = ws_.sync())) break;  // the previous group's pinned staging is rewound below
+    ws_.rewind();
+    rc = decode_batch_group(items + g0, g1 - g0, k, out_ct, max_display_boost, caller);
+    g0 = g1;
+  }
+  if (int r = mark_in_flight()) return rc ? rc : r;
+  if (rc) return rc;
   CUDA_TRY(cudaStreamWaitEvent(caller, writes_done_, 0));
+  return E_OK;
+}
+
+int JpegRCodec::decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller) {
+  const bool sdr_only = out_ct == UHDR_CT_SRGB;
+  int rc = E_OK;
+  // 1. per item, the header stages of both JPEGs (decode_body's order: primary, then map)
+  if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
+  if ((int)batch_idct_.size() < 2 * n) batch_idct_.resize(2 * n);
+  JpegBatchScan* scans = batch_scans_.data();
+  int ns = 0;
+  for (int i = 0; i < n; i++) {
+    DecodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    const DecodedInfo& in = it.info;
+    const bool want_map = it.gainmap || !sdr_only;
+    it.map_rc = E_OK;
+    rc = decode_jpeg_begin(ws_, it.data + in.base_off, in.base_len, sdr_only ? 1 : 0, k, &it.sdr, &it.ph, &it.pj);
+    if (rc == E_MEM) return rc;
+    if (rc) {
+      batch_item_fail(it, rc, last_error());
+      continue;
+    }
+    scans[ns++] = JpegBatchScan{it.data + in.base_off, in.base_len, &it.ph, {}, 0, {0}};
+    if (!want_map) continue;
+    it.map_rc = decode_jpeg_begin(ws_, it.data + in.gainmap_off, in.gainmap_len, 2, k, &it.map, &it.gh, &it.gj);
+    if (it.map_rc == E_MEM) return E_MEM;
+    if (it.map_rc) snprintf(it.map_err, sizeof it.map_err, "%s", last_error());
+    else scans[ns++] = JpegBatchScan{it.data + in.gainmap_off, in.gainmap_len, &it.gh, {}, 0, {0}};
+  }
+  // 2. entropy decoding of every scan
+  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
+  // 3. in the order decode() meets them: the primary's result and its tail stage (which launches nothing for these
+  // modes), the map header's error, the map's result; then one inverse DCT for everything that is left
+  JpegIdctJob* jobs = batch_idct_.data();
+  int nj = 0, si = 0;
+  auto add_job = [&](const JpegHeader& h, const JpegDecodeJob& j, const JpegBatchScan& sc) {
+    JpegIdctJob& o = jobs[nj++];
+    o.h = &h;
+    o.g = j.k != 1 ? &j.g : nullptr;
+    for (int c = 0; c < 3; c++) {
+      o.d_coefs[c] = sc.d_coefs[c];
+      o.planes[c] = j.planes[c];
+      o.strides[c] = j.strides[c];
+    }
+  };
+  for (int i = 0; i < n; i++) {
+    DecodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    const bool want_map = it.gainmap || !sdr_only;
+    const JpegBatchScan& ps = scans[si++];
+    const JpegBatchScan* gs = want_map && !it.map_rc ? &scans[si++] : nullptr;
+    if (ps.rc) {
+      batch_item_fail(it, ps.rc, ps.err);
+      continue;
+    }
+    rc = decode_jpeg_end(ws_, &it.ph, it.pj, &it.sdr, sdr_only ? &it.to_rgba : nullptr);
+    if (rc) {
+      batch_item_fail(it, rc, last_error());
+      continue;
+    }
+    if (it.map_rc) {
+      batch_item_fail(it, it.map_rc, it.map_err);
+      continue;
+    }
+    if (gs && gs->rc) {
+      batch_item_fail(it, gs->rc, gs->err);
+      continue;
+    }
+    add_job(it.ph, it.pj, ps);
+    if (gs) add_job(it.gh, it.gj, *gs);
+  }
+  if (nj && (rc = jpeg_idct_batch_dev(ws_, jobs, nj))) return rc;
+  // 4. per item: the map's tail stage, the gamuts, the metadata, then the writes into the caller's planes
+  if ((rc = join_caller(caller))) return rc;
+  for (int i = 0; i < n; i++) {
+    DecodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    const bool want_map = it.gainmap || !sdr_only;
+    const uint8_t* pd = it.data + it.info.base_off;
+    const uint8_t* gd = it.data + it.info.gainmap_off;
+    ByteView blob = find_marker(pd, it.ph, 0xE2, "ICC_PROFILE", 12);
+    it.sdr.cg = icc_read_gamut(blob.data, blob.size);
+    int r = E_OK;
+    if (want_map) {
+      r = decode_jpeg_end(ws_, &it.gh, it.gj, &it.map, nullptr);
+      if (r == E_MEM) return r;
+      if (!r) {
+        blob = find_marker(gd, it.gh, 0xE2, "ICC_PROFILE", 12);
+        it.map.cg = icc_read_gamut(blob.data, blob.size);
+      }
+    }
+    uhdr_gainmap_metadata_t md{};
+    if (!r && (it.md_out || !sdr_only)) {  // decode_body's metadata step
+      if (!want_map) {
+        r = fail(E_INVALID_PARAM, "received no valid buffer to parse gainmap metadata");
+      } else {
+        const ByteView iso = find_marker(gd, it.gh, 0xE2, "urn:iso:std:iso:ts:21496:-1", 28);
+        const ByteView xmp = find_marker(gd, it.gh, 0xE1, "http://ns.adobe.com/xap/1.0/", 29);
+        const ByteView exif = find_marker(pd, it.ph, 0xE1, "Exif\0\0", 6);
+        r = parse_gainmap_metadata(iso.data, iso.size, xmp.data, xmp.size, exif.data, exif.size, &md);
+        if (!r && it.md_out) *it.md_out = md;
+      }
+    }
+    if (!r) r = check_dev_outputs(it.sdr, it.map, out_ct, it.dest, it.gainmap);
+    if (!r) r = enqueue_dev_writes(it.sdr, it.map, it.to_rgba, md, out_ct, max_display_boost, it.dest, it.gainmap);
+    if (r == E_MEM) return r;
+    if (r) batch_item_fail(it, r, last_error());
+  }
   return E_OK;
 }
 

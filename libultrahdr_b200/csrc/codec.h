@@ -23,6 +23,33 @@ struct DecodedInfo {
   bool has_metadata = false;
 };
 
+// decode_jpeg_dev between its stages (codec.cu): the resolved mode, the scale and the output planes
+struct JpegDecodeJob {
+  int mode = 0, k = 1;
+  JpegScaled g;
+  uint8_t* planes[3] = {nullptr, nullptr, nullptr};
+  int strides[3] = {0, 0, 0};
+};
+
+// One file of JpegRCodec::decode_batch.  The caller fills the first group of fields; rc != E_OK on entry skips the item.
+struct DecodeBatchItem {
+  const uint8_t* data = nullptr;
+  size_t size = 0;
+  DecodedInfo info;  // probe() of the file
+  uhdr_raw_image_t* dest = nullptr;
+  uhdr_raw_image_t* gainmap = nullptr;
+  uhdr_gainmap_metadata_t* md_out = nullptr;
+  int rc = 0;        // out: the code decode() gives for this file alone, its message in err
+  char err[256] = {0};
+  // the decode's state between its batched stages
+  JpegHeader ph, gh;
+  JpegDecodeJob pj, gj;
+  DevImage sdr{}, map{};
+  YccToRgbaParams to_rgba{};
+  int map_rc = 0;    // an error of the gain-map JPEG's header stage, returned after the primary image's own
+  char map_err[256] = {0};
+};
+
 // One parked host thread per codec (spawned on first use, kept until the codec dies): runs the gain-map JPEG of a
 // decode next to the primary one without creating a thread per call.
 class ParkedThread {
@@ -88,6 +115,14 @@ class JpegRCodec {
   // are this codec's scratch, valid until its next call.
   int decode_images(const uint8_t* data, size_t size, const DecodedInfo& probed, int k, DevImage* sdr, DevImage* map,
                     uhdr_gainmap_metadata_t* md);
+  // decode() into device planes (dev_stream, k) of many files, with one entropy decoding and one inverse DCT for all of
+  // them (jpeg_entropy_decode_batch_dev, jpeg_idct_batch_dev), then each file's colour conversion / gain-map
+  // application into its planes.  Each item gets the bytes and the code decode() gives for it alone; a failing item
+  // writes nothing.  Items are taken in groups that fit `group_bytes` of scratch.  The writes are ordered after the
+  // work enqueued earlier on `caller`, which waits for them; settle() waits for them on the host.  The return value is
+  // an error that ends the whole call (CUDA, memory): the items not finished then are left as they were.
+  int decode_batch(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller,
+                   size_t group_bytes);
   // Host wait until what an earlier decode() left in flight is done -- its writes into device planes, or the kernels
   // of a failed call: its scratch (device arenas of both workspaces, the pinned gain tables still waiting for their
   // copy) may be reused after this.
@@ -124,6 +159,16 @@ class JpegRCodec {
   int write_dev_outputs(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
                         const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                         uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, cudaStream_t caller);
+  // write_dev_outputs' parts: the descriptors' checks, the wait for the caller's stream, the writes
+  static int check_dev_outputs(const DevImage& sdr, const DevImage& map, int out_ct, const uhdr_raw_image_t* dest,
+                               const uhdr_raw_image_t* gainmap_out);
+  int join_caller(cudaStream_t caller);
+  int enqueue_dev_writes(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
+                         const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
+                         uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out);
+  int decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller);
+  std::vector<JpegBatchScan> batch_scans_;   // grow-only scratch of decode_batch
+  std::vector<JpegIdctJob> batch_idct_;
   Workspace ws_;
   // second stream + arenas: the gain-map JPEG of a decode is processed by a helper thread while the
   // calling thread handles the primary image (both entropy decoders alternate host and device phases)

@@ -177,11 +177,10 @@ __device__ __forceinline__ void stage_shared(HdShared& S, const HdShared* __rest
   __syncthreads();
 }
 
-// one relaxation round, in place (64-bit states are read and written atomically)
-__global__ void __launch_bounds__(128) k_hd_sync(const uint32_t* __restrict__ bits, unsigned long long* out, unsigned long long* used, unsigned* cnt,
-                                                 unsigned* changed, const HdShared* __restrict__ gs, const HdSeqs q) {
-  __shared__ HdShared S;
-  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+// one relaxation step of subsequence i of the scan whose tables are *gs; a change stores `mark` into *changed
+__device__ __forceinline__ void hd_sync_seq(HdShared& S, const unsigned i, const uint32_t* __restrict__ bits, unsigned long long* out,
+                                            unsigned long long* used, unsigned* cnt, unsigned* changed, const unsigned mark,
+                                            const HdShared* __restrict__ gs, const HdSeqs& q) {
   const unsigned nseq = gs->f.nseq;
   // state word: bit position | (z | c << 8) << 32; an interval's first subsequence starts at its true state
   const unsigned long long entry = i >= nseq ? 0ull
@@ -201,8 +200,28 @@ __global__ void __launch_bounds__(128) k_hd_sync(const uint32_t* __restrict__ bi
   cnt[i] = n;
   if (now != out[i]) {
     *reinterpret_cast<volatile unsigned long long*>(out + i) = now;
-    *changed = 1;
+    *changed = mark;
   }
+}
+
+// one relaxation round, in place (64-bit states are read and written atomically)
+__global__ void __launch_bounds__(128) k_hd_sync(const uint32_t* __restrict__ bits, unsigned long long* out, unsigned long long* used, unsigned* cnt,
+                                                 unsigned* changed, const HdShared* __restrict__ gs, const HdSeqs q) {
+  __shared__ HdShared S;
+  hd_sync_seq(S, blockIdx.x * blockDim.x + threadIdx.x, bits, out, used, cnt, changed, 1u, gs, q);
+}
+
+// start bit of subsequence i < nseq and its interval *iv
+__device__ __forceinline__ unsigned hd_seq_lo(const unsigned* __restrict__ start, const unsigned* __restrict__ first, unsigned nint,
+                                              unsigned i, unsigned* iv) {
+  unsigned a = 0, b = nint - 1;  // last interval whose first subsequence is <= i
+  while (a < b) {
+    const unsigned m = (a + b + 1) / 2;
+    if (first[m] <= i) a = m;
+    else b = m - 1;
+  }
+  *iv = a;
+  return start[a] + (i - first[a]) * (unsigned)kSeqBits;
 }
 
 // expands the per-interval layout built on the host (start bit and first subsequence of each interval)
@@ -212,14 +231,7 @@ __global__ void k_hd_layout(const unsigned* __restrict__ start, const unsigned* 
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) lo[nseq] = total_bits;
   if (i >= nseq) return;
-  unsigned a = 0, b = nint - 1;  // last interval whose first subsequence is <= i
-  while (a < b) {
-    const unsigned m = (a + b + 1) / 2;
-    if (first[m] <= i) a = m;
-    else b = m - 1;
-  }
-  lo[i] = start[a] + (i - first[a]) * (unsigned)kSeqBits;
-  iv[i] = a;
+  lo[i] = hd_seq_lo(start, first, nint, i, iv + i);
 }
 
 __global__ void k_hd_init(unsigned long long* out, unsigned long long* used, unsigned* cnt, unsigned nseq, const unsigned* __restrict__ lo) {
@@ -231,7 +243,7 @@ __global__ void k_hd_init(unsigned long long* out, unsigned long long* used, uns
 }
 
 // exclusive prefix sum of cnt (one CTA; nseq is at most a few hundred thousand)
-__global__ void __launch_bounds__(1024) k_hd_scan(const unsigned* __restrict__ cnt, unsigned* __restrict__ base, unsigned n) {
+__device__ __forceinline__ void hd_prefix(const unsigned* __restrict__ cnt, unsigned* __restrict__ base, unsigned n) {
   __shared__ unsigned warp_sums[32];
   __shared__ unsigned carry;
   if (threadIdx.x == 0) carry = 0;
@@ -262,13 +274,15 @@ __global__ void __launch_bounds__(1024) k_hd_scan(const unsigned* __restrict__ c
     __syncthreads();
   }
 }
+__global__ void __launch_bounds__(1024) k_hd_scan(const unsigned* __restrict__ cnt, unsigned* __restrict__ base, unsigned n) {
+  hd_prefix(cnt, base, n);
+}
 
-// out and base are read only for subsequences that do not start an interval
-__global__ void __launch_bounds__(128) k_hd_write(const uint32_t* __restrict__ bits, const unsigned long long* __restrict__ out, const unsigned* __restrict__ base,
-                                                  const HdShared* __restrict__ gs, const HdSeqs q, HdOut o) {
-  __shared__ HdShared S;
-  stage_shared(S, gs);
-  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+// the writing pass for subsequence i, tables staged in S.  out and base are read only for subsequences that do not
+// start an interval
+__device__ __forceinline__ void hd_write_seq(const HdShared& S, const unsigned i, const uint32_t* __restrict__ bits,
+                                             const unsigned long long* __restrict__ out, const unsigned* __restrict__ base,
+                                             const HdSeqs& q, const HdOut& o) {
   if (i >= S.f.nseq) return;
   const unsigned k = q.iv[i], head = q.first[k], next = q.first[k + 1];
   const unsigned long long entry = head == i ? (unsigned long long)q.lo[i] : out[i - 1];
@@ -279,6 +293,80 @@ __global__ void __launch_bounds__(128) k_hd_write(const uint32_t* __restrict__ b
   if (b % (unsigned)S.f.bpm != c) *o.err = 2;  // the states and the block counts must agree
   const unsigned n = decode_seq<true>(S, bits, p, z, c, q.lo[i + 1], b, b_end, q.lo[next], o);
   if (next == i + 1 && b + n < b_end) *o.err = 1;  // the interval holds fewer blocks than it must
+}
+__global__ void __launch_bounds__(128) k_hd_write(const uint32_t* __restrict__ bits, const unsigned long long* __restrict__ out, const unsigned* __restrict__ base,
+                                                  const HdShared* __restrict__ gs, const HdSeqs q, HdOut o) {
+  __shared__ HdShared S;
+  stage_shared(S, gs);
+  hd_write_seq(S, blockIdx.x * blockDim.x + threadIdx.x, bits, out, base, q, o);
+}
+
+// ---- a batch of scans (jpeg_entropy_decode_batch_dev) ----
+// Scan s owns subsequence slots [seq0, seq0 + nseq + 1) of the batch's per-subsequence arrays, seq0 a multiple of
+// 128, so that every CTA of the relaxation and writing passes works on one scan and stages one scan's tables; and
+// intervals [iv0, iv0 + nint + 1) of its per-interval arrays.  Within its slice a scan is laid out as alone.
+struct HdScan {
+  const uint32_t* bits;
+  unsigned seq0, iv0, nint;
+  HdOut o;
+};
+struct HdBatch {
+  const HdShared* gs;     // per scan
+  const HdScan* scans;
+  const uint2* ctas;      // per CTA of a launch: {scan, first slot}
+  const unsigned* start;  // per interval: start bit (local to the scan)
+  HdSeqs q;               // lo / iv / first of every scan, values local to the scan
+};
+__device__ __forceinline__ HdSeqs hd_local(const HdBatch& B, const HdScan& sc) {
+  return HdSeqs{B.q.lo + sc.seq0, B.q.iv + sc.seq0, B.q.first + sc.iv0};
+}
+
+// k_hd_layout and k_hd_init of every scan in one launch, one thread per slot
+__global__ void __launch_bounds__(128) k_hd_layout_batch(const HdBatch B, unsigned* lo, unsigned* iv, unsigned long long* out,
+                                                         unsigned long long* used, unsigned* cnt) {
+  const uint2 cta = B.ctas[blockIdx.x];
+  const HdScan& sc = B.scans[cta.x];
+  const unsigned nseq = B.gs[cta.x].f.nseq, total_bits = B.gs[cta.x].f.total_bits;
+  const unsigned i = cta.y - sc.seq0 + threadIdx.x;
+  const HdSeqs q = hd_local(B, sc);
+  const unsigned* start = B.start + sc.iv0;
+  if (i == 0) lo[sc.seq0 + nseq] = total_bits;
+  if (i >= nseq) return;
+  unsigned iv1;
+  lo[sc.seq0 + i] = hd_seq_lo(start, q.first, sc.nint, i, iv + sc.seq0 + i);
+  out[sc.seq0 + i] = i + 1 < nseq ? (unsigned long long)hd_seq_lo(start, q.first, sc.nint, i + 1, &iv1) : (unsigned long long)total_bits;
+  used[sc.seq0 + i] = ~0ull;
+  cnt[sc.seq0 + i] = 0;
+}
+
+// one relaxation round over the CTAs of the scans that still need rounds; a scan's change stores round + 1 into
+// last[scan]
+__global__ void __launch_bounds__(128) k_hd_sync_batch(const HdBatch B, unsigned long long* out, unsigned long long* used, unsigned* cnt,
+                                                       unsigned* last, const unsigned round) {
+  __shared__ HdShared S;
+  const uint2 cta = B.ctas[blockIdx.x];
+  const HdScan& sc = B.scans[cta.x];
+  const unsigned seq0 = sc.seq0;
+  hd_sync_seq(S, cta.y - seq0 + threadIdx.x, sc.bits, out + seq0, used + seq0, cnt + seq0, last + cta.x, round + 1, B.gs + cta.x,
+              hd_local(B, sc));
+}
+
+// k_hd_scan of each scan that had rounds: one CTA per scan
+__global__ void __launch_bounds__(1024) k_hd_scan_batch(const HdBatch B, const unsigned* __restrict__ which, const unsigned* __restrict__ cnt,
+                                                        unsigned* __restrict__ base) {
+  const unsigned s = which[blockIdx.x];
+  const unsigned seq0 = B.scans[s].seq0;
+  hd_prefix(cnt + seq0, base + seq0, B.gs[s].f.nseq);
+}
+
+__global__ void __launch_bounds__(128) k_hd_write_batch(const HdBatch B, const unsigned long long* __restrict__ out,
+                                                        const unsigned* __restrict__ base) {
+  __shared__ HdShared S;
+  const uint2 cta = B.ctas[blockIdx.x];
+  stage_shared(S, B.gs + cta.x);
+  const HdScan& sc = B.scans[cta.x];
+  const unsigned seq0 = sc.seq0;
+  hd_write_seq(S, cta.y - seq0 + threadIdx.x, sc.bits, out + seq0, base + seq0, hd_local(B, sc), sc.o);
 }
 
 // ---- DC prediction: inclusive scan of the differences per component, scatter into the blocks ----
@@ -310,14 +398,15 @@ __device__ __forceinline__ int cta_inclusive_scan(int v, int* warp_sums /* [32] 
   __syncthreads();
   return x + ((threadIdx.x >> 5) ? warp_sums[(threadIdx.x >> 5) - 1] : 0);
 }
-__global__ void __launch_bounds__(kDcCta) k_dc_local(DcPlan d) {
+__device__ __forceinline__ void dc_local(const DcPlan& d, const unsigned cta) {
   __shared__ int ws[32];
-  const unsigned i = blockIdx.x * kDcCta + threadIdx.x;
+  const unsigned i = cta * kDcCta + threadIdx.x;
   const int x = cta_inclusive_scan(i < d.n ? d.dcd[i] : 0, ws);
   if (i < d.n) d.dcd[i] = x;
-  if (threadIdx.x == kDcCta - 1) d.sums[blockIdx.x] = x;
+  if (threadIdx.x == kDcCta - 1) d.sums[cta] = x;
 }
-__global__ void __launch_bounds__(kDcCta) k_dc_sums(int* sums, unsigned n) {  // in place, exclusive, one CTA
+__global__ void __launch_bounds__(kDcCta) k_dc_local(DcPlan d) { dc_local(d, blockIdx.x); }
+__device__ __forceinline__ void dc_sums(int* sums, unsigned n) {  // in place, exclusive, one CTA
   __shared__ int ws[32];
   __shared__ int carry;
   if (threadIdx.x == 0) carry = 0;
@@ -332,8 +421,8 @@ __global__ void __launch_bounds__(kDcCta) k_dc_sums(int* sums, unsigned n) {  //
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(256) k_dc_apply(DcPlan d) {
-  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void __launch_bounds__(kDcCta) k_dc_sums(int* sums, unsigned n) { dc_sums(sums, n); }
+__device__ __forceinline__ void dc_apply(const DcPlan& d, const unsigned i) {
   if (i >= d.n) return;
   // running sum within the interval = prefix sum to i minus prefix sum before the interval's first block;
   // exact in wrapping 32-bit arithmetic, which is how jpeg_host_decode_coefs accumulates too
@@ -344,6 +433,23 @@ __global__ void __launch_bounds__(256) k_dc_apply(DcPlan d) {
   const int bx = (int)(mcu % (unsigned)d.mcus_per_row) * d.h + (int)(k % (unsigned)d.h);
   const int by = (int)(mcu / (unsigned)d.mcus_per_row) * d.v + (int)(k / (unsigned)d.h);
   if (bx < d.wblocks && by < d.hblocks) d.coefs[((size_t)by * d.wblocks + bx) * 64] = (int16_t)dc;
+}
+__global__ void __launch_bounds__(256) k_dc_apply(DcPlan d) { dc_apply(d, blockIdx.x * blockDim.x + threadIdx.x); }
+
+// The three DC passes over many plans (every component of every scan of a batch), one launch each.  cta_end[j]: the
+// CTAs of plans 0..j in the launch's numbering (inclusive prefix), kDcCta-thread CTAs for the local pass, 256-thread
+// ones for the scatter; the sums pass runs one CTA per plan.
+__global__ void __launch_bounds__(kDcCta) k_dc_local_batch(const DcPlan* __restrict__ plans, const unsigned* __restrict__ cta_end, unsigned n) {
+  const unsigned j = batch_find(cta_end, n, blockIdx.x);
+  dc_local(plans[j], blockIdx.x - (j ? cta_end[j - 1] : 0));
+}
+__global__ void __launch_bounds__(kDcCta) k_dc_sums_batch(const DcPlan* __restrict__ plans) {
+  const DcPlan& d = plans[blockIdx.x];
+  dc_sums(d.sums, (d.n + kDcCta - 1) / kDcCta);
+}
+__global__ void __launch_bounds__(256) k_dc_apply_batch(const DcPlan* __restrict__ plans, const unsigned* __restrict__ cta_end, unsigned n) {
+  const unsigned j = batch_find(cta_end, n, blockIdx.x);
+  dc_apply(plans[j], (blockIdx.x - (j ? cta_end[j - 1] : 0)) * 256 + threadIdx.x);
 }
 
 void build_tables(const JpegHeader& h, HdTables* t) {
@@ -422,9 +528,10 @@ static long unstuff_scan(const uint8_t* data, size_t size, size_t from, uint8_t*
   return k == nint ? (long)(o - dst) : -1;
 }
 
-int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, const JpegHeader& h, int16_t* d_coefs[3]) {
+// The frame description and tables of a scan (all of hs but total_bits and nseq), its MCUs per restart interval and
+// its intervals; kHuffDecFallback for a scan the device decoder does not take
+static int hd_prepare(const JpegHeader& h, HdShared& hs, size_t* ri_out, unsigned* nint_out) {
   const JpegFrame& f = h.frame;
-  HdShared hs;
   memset(&hs, 0, sizeof hs);
   HdFrame& hf = hs.f;
   int bpm = 0;
@@ -461,6 +568,50 @@ int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, con
   const unsigned nint = (unsigned)((mcus + ri - 1) / ri);
   hf.iv_blocks = (unsigned)(ri * bpm);
   build_tables(h, &hs.t);
+  *ri_out = ri;
+  *nint_out = nint;
+  return E_OK;
+}
+
+// subsequences: every interval is cut into pieces of at most kSeqBits bits (an empty interval gets one empty piece,
+// whose missing blocks the writing pass reports).  The host numbers them per interval (starts: clean byte offsets in,
+// bit offsets out; first[k]: the interval's first subsequence); k_hd_layout expands that on the device.  Returns nseq.
+static unsigned hd_intervals(unsigned* starts, unsigned* first, unsigned nint, unsigned total_bits) {
+  size_t nseq_total = 0;
+  for (unsigned k = 0; k < nint; k++) {
+    const unsigned lo = starts[k] * 8u, hi = k + 1 < nint ? starts[k + 1] * 8u : total_bits;
+    starts[k] = lo;
+    first[k] = (unsigned)nseq_total;
+    nseq_total += hi > lo ? (hi - lo + kSeqBits - 1) / kSeqBits : 1;
+  }
+  first[nint] = (unsigned)nseq_total;
+  return (unsigned)nseq_total;
+}
+
+// kZigzagDev: once per device, synchronously and under a lock (decodes run concurrently on several streams / threads)
+static int upload_zigzag() {
+  static std::mutex zig_mu;
+  static bool zig_done[64] = {false};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lk(zig_mu);
+  if (dev < 0 || dev >= 64 || !zig_done[dev]) {
+    void* zig = nullptr;
+    CUDA_TRY(cudaGetSymbolAddress(&zig, kZigzagDev));
+    if (int rc = copy_sync(zig, kZigzag, 64, cudaMemcpyHostToDevice)) return rc;
+    if (dev >= 0 && dev < 64) zig_done[dev] = true;
+  }
+  return E_OK;
+}
+
+int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, const JpegHeader& h, int16_t* d_coefs[3]) {
+  const JpegFrame& f = h.frame;
+  HdShared hs;
+  HdFrame& hf = hs.f;
+  size_t ri = 0;
+  unsigned nint = 0;
+  if (int rc = hd_prepare(h, hs, &ri, &nint)) return rc;
+  const size_t mcus = (size_t)f.mcus_per_row * f.mcu_rows;
 
   // 1. clean bit stream in pinned memory, then on the device (8 zero bytes of slack for the reader)
   if (size <= h.scan_offset) return fail(E_ERROR, "Corrupt JPEG data: no entropy-coded segment");
@@ -478,20 +629,9 @@ int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, con
   hf.total_bits = (unsigned)(clean * 8);
   if (hf.total_bits == 0) return fail(E_ERROR, "Corrupt JPEG data: empty entropy-coded segment");
 
-  // subsequences: every interval is cut into pieces of at most kSeqBits bits (an empty interval
-  // gets one empty piece, whose missing blocks the writing pass reports).  The host numbers them per
-  // interval; k_hd_layout expands that on the device.
   unsigned* h_first = (unsigned*)ws.halloc(sizeof(unsigned) * (nint + 1));
   if (!h_first) return E_MEM;
-  size_t nseq_total = 0;
-  for (unsigned k = 0; k < nint; k++) {
-    const unsigned lo = h_starts[k] * 8u, hi = k + 1 < nint ? h_starts[k + 1] * 8u : hf.total_bits;
-    h_starts[k] = lo;
-    h_first[k] = (unsigned)nseq_total;
-    nseq_total += hi > lo ? (hi - lo + kSeqBits - 1) / kSeqBits : 1;
-  }
-  const unsigned nseq = (unsigned)nseq_total;
-  h_first[nint] = nseq;
+  const unsigned nseq = hd_intervals(h_starts, h_first, nint, hf.total_bits);
   hf.nseq = nseq;
   tr.mark("  interval layout");
 
@@ -520,19 +660,7 @@ int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, con
   k_hd_layout<<<(nseq + 255) / 256, 256, 0, s>>>(d_start, d_first, nint, nseq, hf.total_bits, d_lo, d_iv);
   count_launches(1);
   CUDA_TRY(cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (kMaxRounds + 8), s));
-  {  // once per device, synchronously and under a lock: decodes run concurrently on several streams / threads
-    static std::mutex zig_mu;
-    static bool zig_done[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(zig_mu);
-    if (dev < 0 || dev >= 64 || !zig_done[dev]) {
-      void* zig = nullptr;
-      CUDA_TRY(cudaGetSymbolAddress(&zig, kZigzagDev));
-      if (int rc = copy_sync(zig, kZigzag, 64, cudaMemcpyHostToDevice)) return rc;
-      if (dev >= 0 && dev < 64) zig_done[dev] = true;
-    }
-  }
+  if (int rc = upload_zigzag()) return rc;
   // coefficient blocks start as zeros; only non-zero coefficients are written
   int* d_dcd[3] = {nullptr, nullptr, nullptr};
   for (int c = 0; c < f.ncomp; c++) {
@@ -608,6 +736,250 @@ int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, con
   if (h_flags[0]) return declined();  // let the host decoder produce the diagnosis
   g_hd_done.fetch_add(1);
   g_hd_rounds.store((unsigned long long)first_quiet);
+  return E_OK;
+}
+
+namespace {
+template <typename T>
+T* dalloc_n(Workspace& ws, size_t n) { return (T*)ws.dalloc(sizeof(T) * (n ? n : 1)); }
+template <typename T>
+T* halloc_n(Workspace& ws, size_t n) { return (T*)ws.halloc(sizeof(T) * (n ? n : 1)); }
+void scan_error(JpegBatchScan& sc, int rc) {
+  sc.rc = rc;
+  snprintf(sc.err, sizeof sc.err, "%s", last_error());
+}
+}  // namespace
+
+int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
+  cudaStream_t s = ws.stream();
+  struct Plan {
+    bool dev;              // on the device (else the host decoder)
+    bool relax;            // has relaxation rounds
+    unsigned nint, nseq, seq0, iv0;
+    size_t ri, bits_off;   // bits_off: clean bytes before this scan's in the staging buffer (multiple of 4)
+  };
+  Plan* pl = halloc_n<Plan>(ws, n);
+  HdShared* h_hs = halloc_n<HdShared>(ws, n);
+  if (!pl || !h_hs) return E_MEM;
+  // 1. per scan, on the host: tables, intervals, and the staging size of its clean bits
+  size_t bits_cap = 0, niv = 0;
+  for (int i = 0; i < n; i++) {
+    JpegBatchScan& sc = scans[i];
+    const JpegHeader& h = *sc.h;
+    Plan& p = pl[i];
+    memset(&p, 0, sizeof p);
+    sc.rc = E_OK;
+    for (int c = 0; c < 3; c++) sc.d_coefs[c] = nullptr;
+    p.dev = hd_prepare(h, h_hs[i], &p.ri, &p.nint) == E_OK;
+    if (!p.dev) continue;
+    if (sc.size <= h.scan_offset) {
+      scan_error(sc, fail(E_ERROR, "Corrupt JPEG data: no entropy-coded segment"));
+      continue;
+    }
+    p.bits_off = bits_cap;
+    p.iv0 = (unsigned)niv;
+    bits_cap += (sc.size - h.scan_offset + 16 + 3) & ~(size_t)3;
+    niv += p.nint + 1;
+  }
+  uint8_t* h_bits = halloc_n<uint8_t>(ws, bits_cap);
+  unsigned* h_start = halloc_n<unsigned>(ws, niv);
+  unsigned* h_first = halloc_n<unsigned>(ws, niv);
+  if (!h_bits || !h_start || !h_first) return E_MEM;
+  // 2. every scan unstuffed into one pinned buffer; a scan with irregular restart markers goes to the host decoder
+  size_t nslots = 0, nrelax = 0, cta_all = 0, cta_sync = 0;
+  for (int i = 0; i < n; i++) {
+    JpegBatchScan& sc = scans[i];
+    Plan& p = pl[i];
+    if (!p.dev || sc.rc) continue;
+    uint8_t* dst = h_bits + p.bits_off;
+    const long clean = unstuff_scan(sc.data, sc.size, sc.h->scan_offset, dst, sc.h->restart_interval != 0, h_start + p.iv0, p.nint);
+    if (clean < 0 || (size_t)clean * 8 > 0xfffffff0u - kSeqBits) {
+      p.dev = false;
+      declined();
+      continue;
+    }
+    memset(dst + clean, 0, 16);
+    HdFrame& hf = h_hs[i].f;
+    hf.total_bits = (unsigned)(clean * 8);
+    if (hf.total_bits == 0) {
+      scan_error(sc, fail(E_ERROR, "Corrupt JPEG data: empty entropy-coded segment"));
+      continue;
+    }
+    p.nseq = hf.nseq = hd_intervals(h_start + p.iv0, h_first + p.iv0, p.nint, hf.total_bits);
+    p.relax = p.nseq > p.nint;
+    p.seq0 = (unsigned)nslots;
+    nslots += (p.nseq + 1 + 127) / 128 * 128;  // + 1: lo[nseq]
+    const unsigned ctas = (p.nseq + 127) / 128;
+    cta_all += ctas;
+    if (p.relax) {
+      cta_sync += ctas;
+      nrelax++;
+    }
+  }
+  if (nslots > 0xffffff00u) return fail(E_ERROR, "internal: entropy-decoder batch of %zu subsequences", nslots);
+  // the CTA lists (all scans, then those with rounds), the scans with rounds, the per-scan slices, the DC plans
+  uint2* h_ctas = halloc_n<uint2>(ws, cta_all + cta_sync);
+  unsigned* h_which = halloc_n<unsigned>(ws, nrelax);
+  HdScan* h_scans = halloc_n<HdScan>(ws, n);
+  unsigned* h_last = halloc_n<unsigned>(ws, 2 * (size_t)n);  // [0, n): last changing round, [n, 2n): write-pass errors
+  DcPlan* h_dc = halloc_n<DcPlan>(ws, 3 * (size_t)n);
+  unsigned* h_dc_end = halloc_n<unsigned>(ws, 6 * (size_t)n);  // [0, 3n): local-pass CTAs, [3n, 6n): scatter CTAs
+  if (!h_ctas || !h_which || !h_scans || !h_last || !h_dc || !h_dc_end) return E_MEM;
+  uint32_t* d_bits = dalloc_n<uint32_t>(ws, bits_cap / 4);
+  HdShared* d_hs = dalloc_n<HdShared>(ws, n);
+  HdScan* d_scans = dalloc_n<HdScan>(ws, n);
+  uint2* d_ctas = dalloc_n<uint2>(ws, cta_all + cta_sync);
+  unsigned* d_which = dalloc_n<unsigned>(ws, nrelax);
+  unsigned* d_start = dalloc_n<unsigned>(ws, niv);
+  unsigned* d_first = dalloc_n<unsigned>(ws, niv);
+  unsigned* d_lo = dalloc_n<unsigned>(ws, nslots);
+  unsigned* d_iv = dalloc_n<unsigned>(ws, nslots);
+  unsigned long long* d_out = dalloc_n<unsigned long long>(ws, nslots);
+  unsigned long long* d_used = dalloc_n<unsigned long long>(ws, nslots);
+  unsigned* d_cnt = dalloc_n<unsigned>(ws, nslots);
+  unsigned* d_base = dalloc_n<unsigned>(ws, nslots);
+  unsigned* d_last = dalloc_n<unsigned>(ws, 2 * (size_t)n);
+  DcPlan* d_dc = dalloc_n<DcPlan>(ws, 3 * (size_t)n);
+  unsigned* d_dc_end = dalloc_n<unsigned>(ws, 6 * (size_t)n);
+  if (!d_bits || !d_hs || !d_scans || !d_ctas || !d_which || !d_start || !d_first || !d_lo || !d_iv || !d_out || !d_used || !d_cnt ||
+      !d_base || !d_last || !d_dc || !d_dc_end)
+    return E_MEM;
+  // coefficient blocks start as zeros (the device decoder writes only non-zero coefficients; the host decoder's
+  // blocks are copied over them)
+  size_t a = 0, b = 0, nw = 0, ndc = 0, n_local = 0, n_apply = 0;
+  for (int i = 0; i < n; i++) {
+    JpegBatchScan& sc = scans[i];
+    const Plan& p = pl[i];
+    if (sc.rc) continue;
+    const JpegFrame& f = sc.h->frame;
+    const HdFrame& hf = h_hs[i].f;
+    HdScan& hs = h_scans[i];
+    memset(&hs, 0, sizeof hs);
+    for (int c = 0; c < f.ncomp; c++) {
+      sc.d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
+      if (!sc.d_coefs[c]) return E_MEM;
+      CUDA_TRY(cudaMemsetAsync(sc.d_coefs[c], 0, f.blocks(c) * 128, s));
+    }
+    if (!p.dev) continue;
+    hs.bits = d_bits + p.bits_off / 4;
+    hs.seq0 = p.seq0;
+    hs.iv0 = p.iv0;
+    hs.nint = p.nint;
+    hs.o.err = d_last + n + i;
+    const size_t mcus = (size_t)f.mcus_per_row * f.mcu_rows;
+    for (int c = 0; c < f.ncomp; c++) {
+      hs.o.coefs[c] = sc.d_coefs[c];
+      hs.o.dcd[c] = (int*)ws.dalloc(sizeof(int) * mcus * hf.hv[c]);
+      if (!hs.o.dcd[c]) return E_MEM;
+      DcPlan& d = h_dc[ndc];
+      d.dcd = hs.o.dcd[c];
+      d.coefs = sc.d_coefs[c];
+      d.n = (unsigned)(mcus * hf.hv[c]);
+      d.seg = (unsigned)(p.ri * hf.hv[c]);
+      d.h = hf.h[c]; d.v = hf.v[c]; d.hv = hf.hv[c];
+      d.wblocks = hf.wblocks[c]; d.hblocks = hf.hblocks[c];
+      d.mcus_per_row = hf.mcus_per_row;
+      const unsigned nct = (d.n + kDcCta - 1) / kDcCta;
+      d.sums = (int*)ws.dalloc(sizeof(int) * nct);
+      if (!d.sums) return E_MEM;
+      n_local += nct;
+      n_apply += (d.n + 255) / 256;
+      h_dc_end[ndc] = (unsigned)n_local;
+      h_dc_end[3 * n + ndc] = (unsigned)n_apply;
+      ndc++;
+    }
+    const unsigned ctas = (p.nseq + 127) / 128;
+    for (unsigned c = 0; c < ctas; c++) {
+      h_ctas[a++] = make_uint2((unsigned)i, p.seq0 + c * 128);
+      if (p.relax) h_ctas[cta_all + b++] = make_uint2((unsigned)i, p.seq0 + c * 128);
+    }
+    if (p.relax) h_which[nw++] = (unsigned)i;
+  }
+  if (cta_all) {
+    CUDA_TRY(cudaMemcpyAsync(d_bits, h_bits, bits_cap, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_hs, h_hs, sizeof(HdShared) * n, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_scans, h_scans, sizeof(HdScan) * n, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_ctas, h_ctas, sizeof(uint2) * (cta_all + cta_sync), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_which, h_which, sizeof(unsigned) * (nrelax ? nrelax : 1), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_start, h_start, sizeof(unsigned) * niv, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_first, h_first, sizeof(unsigned) * niv, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_dc, h_dc, sizeof(DcPlan) * ndc, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(d_dc_end, h_dc_end, sizeof(unsigned) * 6 * n, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemsetAsync(d_last, 0, sizeof(unsigned) * 2 * n, s));
+    if (int rc = upload_zigzag()) return rc;
+    HdBatch B = {d_hs, d_scans, d_ctas, d_start, HdSeqs{d_lo, d_iv, d_first}};
+    k_hd_layout_batch<<<(unsigned)cta_all, 128, 0, s>>>(B, d_lo, d_iv, d_out, d_used, d_cnt);
+    count_launches(1);
+    CUDA_TRY(cudaGetLastError());
+    // 3. relaxation rounds over every scan that has them, one host check per kRoundsPerBatch rounds for the whole
+    // batch, until each of them has had a round that changed nothing
+    int rounds = 0;
+    bool pending = cta_sync > 0;
+    HdBatch Bs = B;
+    Bs.ctas = d_ctas + cta_all;
+    if (pending) ws.t_begin("huffdec_sync_batch");
+    while (pending && rounds < kMaxRounds) {
+      count_launches(kRoundsPerBatch);
+      for (int r = 0; r < kRoundsPerBatch; r++)
+        k_hd_sync_batch<<<(unsigned)cta_sync, 128, 0, s>>>(Bs, d_out, d_used, d_cnt, d_last, (unsigned)(rounds + r));
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(cudaMemcpyAsync(h_last, d_last, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, s));
+      CUDA_TRY(cudaStreamSynchronize(s));
+      rounds += kRoundsPerBatch;
+      pending = false;
+      for (size_t j = 0; j < nrelax; j++) pending = pending || h_last[h_which[j]] == (unsigned)rounds;  // changed in the last round
+    }
+    if (cta_sync) ws.t_end();
+    for (size_t j = 0; j < nrelax; j++) {
+      const unsigned i = h_which[j];
+      if (h_last[i] == (unsigned)rounds) {  // no quiet round in kMaxRounds: the host decoder takes it
+        pl[i].dev = false;
+        declined();
+      } else {
+        g_hd_rounds.store((unsigned long long)h_last[i] + 1);  // the first quiet round
+      }
+    }
+    // 4. block offsets within each interval, the writing pass, DC prediction: one launch each for the batch
+    ws.t_begin("huffdec_write_batch");
+    if (nrelax) k_hd_scan_batch<<<(unsigned)nrelax, 1024, 0, s>>>(B, d_which, d_cnt, d_base);
+    k_hd_write_batch<<<(unsigned)cta_all, 128, 0, s>>>(B, d_out, d_base);
+    ws.t_end();
+    ws.t_begin("huffdec_dc_batch");
+    k_dc_local_batch<<<(unsigned)n_local, kDcCta, 0, s>>>(d_dc, d_dc_end, (unsigned)ndc);
+    k_dc_sums_batch<<<(unsigned)ndc, kDcCta, 0, s>>>(d_dc);
+    k_dc_apply_batch<<<(unsigned)n_apply, 256, 0, s>>>(d_dc, d_dc_end + 3 * n, (unsigned)ndc);
+    ws.t_end();
+    count_launches((nrelax ? 1 : 0) + 4);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(h_last + n, d_last + n, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    for (int i = 0; i < n; i++) {
+      if (!pl[i].dev || scans[i].rc) continue;
+      if (h_last[n + i]) {  // let the host decoder produce the diagnosis
+        pl[i].dev = false;
+        declined();
+      } else {
+        g_hd_done.fetch_add(1);
+      }
+    }
+  }
+  // 5. the scans the device decoder did not take, on the host; their blocks replace the device's
+  for (int i = 0; i < n; i++) {
+    JpegBatchScan& sc = scans[i];
+    if (pl[i].dev || sc.rc) continue;
+    const JpegFrame& f = sc.h->frame;
+    int16_t* h_coefs[3] = {nullptr, nullptr, nullptr};
+    for (int c = 0; c < f.ncomp; c++) {
+      h_coefs[c] = (int16_t*)ws.halloc(f.blocks(c) * 128);
+      if (!h_coefs[c]) return E_MEM;
+    }
+    if (int rc = jpeg_host_decode_coefs(sc.data, sc.size, *sc.h, h_coefs)) {
+      scan_error(sc, rc);
+      continue;
+    }
+    for (int c = 0; c < f.ncomp; c++)
+      CUDA_TRY(cudaMemcpyAsync(sc.d_coefs[c], h_coefs[c], f.blocks(c) * 128, cudaMemcpyHostToDevice, s));
+  }
   return E_OK;
 }
 

@@ -7,7 +7,8 @@
 //    k_idct_dequant; +128 and a saturating clamp, the semantics of the SIMD forms the library runs.
 //  - 1x1: (dc * q0 + 4) >> 3 through the C range-limit table (the library has no SIMD form of it): the value is read
 //    modulo 1024 as a signed number, then +128 and clamped.
-// One thread per block; one launch covers every plane of a JPEG whose DCT scaled size is S.
+// One thread per block; one launch covers every plane of a JPEG whose DCT scaled size is S (k_idct_scaled_batch: of
+// many JPEGs).
 #include "kernels.cuh"
 
 namespace uhdr_b200 {
@@ -47,22 +48,12 @@ __device__ __forceinline__ void load_row(const int16_t* blk, const uint16_t* q, 
   for (int k = 0; k < 8; k++) v[k] = (int)(int16_t)((w[k >> 1] >> ((k & 1) * 16)) & 0xffff) * (int)q[r * 8 + k];
 }
 
+// block `local` of a plane, quantiser q in shared memory
 template <int S>
-__global__ void __launch_bounds__(128) k_idct_scaled(const __grid_constant__ IdctScaledParams p) {
-  __shared__ uint16_t sq[3][64];
-  for (int i = threadIdx.x; i < p.nplanes * 64; i += blockDim.x) sq[i >> 6][i & 63] = p.plane[i >> 6].q[i & 63];
-  __syncthreads();
-  const int gb = blockIdx.x * blockDim.x + threadIdx.x;
-  if (gb >= p.block_end[p.nplanes - 1]) return;
-  const int c = gb < p.block_end[0] ? 0 : gb < p.block_end[1] ? 1 : 2;
-  const IdctScaledParams::Plane& pl = p.plane[c];  // __grid_constant__: read in place, no local copy
-  const int16_t* coefs = pl.coefs;
-  uint8_t* dst = pl.dst;
-  const int wblocks = pl.wblocks, stride = pl.dst_stride, dst_w = pl.dst_w, dst_h = pl.dst_h;
-  const int local = gb - (c == 0 ? 0 : p.block_end[c - 1]);
+__device__ __forceinline__ void idct_scaled_block(const int16_t* coefs, const uint16_t* q, int local, int wblocks, uint8_t* dst, int stride,
+                                                  int dst_w, int dst_h) {
   const int by = local / wblocks, bx = local - by * wblocks;
   const int16_t* blk = coefs + (size_t)local * 64;
-  const uint16_t* q = sq[c];
   uint8_t* out = dst + (size_t)by * S * stride + bx * S;
   if (S == 1) {
     if (by >= dst_h || bx >= dst_w) return;
@@ -122,7 +113,46 @@ __global__ void __launch_bounds__(128) k_idct_scaled(const __grid_constant__ Idc
   }
 }
 
+template <int S>
+__global__ void __launch_bounds__(128) k_idct_scaled(const __grid_constant__ IdctScaledParams p) {
+  __shared__ uint16_t sq[3][64];
+  for (int i = threadIdx.x; i < p.nplanes * 64; i += blockDim.x) sq[i >> 6][i & 63] = p.plane[i >> 6].q[i & 63];
+  __syncthreads();
+  const int gb = blockIdx.x * blockDim.x + threadIdx.x;
+  if (gb >= p.block_end[p.nplanes - 1]) return;
+  const int c = gb < p.block_end[0] ? 0 : gb < p.block_end[1] ? 1 : 2;
+  const IdctScaledParams::Plane& pl = p.plane[c];  // __grid_constant__: read in place, no local copy
+  idct_scaled_block<S>(pl.coefs, sq[c], gb - (c == 0 ? 0 : p.block_end[c - 1]), pl.wblocks, pl.dst, pl.dst_stride, pl.dst_w, pl.dst_h);
+}
+
+// every plane of a batch in one launch: each CTA covers 128 blocks of one plane
+template <int S>
+__global__ void __launch_bounds__(128) k_idct_scaled_batch(const IdctBatchPlane* __restrict__ planes, const unsigned* __restrict__ cta_end,
+                                                           unsigned n) {
+  const unsigned j = batch_find(cta_end, n, blockIdx.x);
+  const IdctBatchPlane& p = planes[j];
+  __shared__ uint16_t sq[64];
+  if (threadIdx.x < 64) sq[threadIdx.x] = p.q[threadIdx.x];
+  __syncthreads();
+  const int local = (int)(blockIdx.x - (j ? cta_end[j - 1] : 0)) * 128 + threadIdx.x;
+  if (local >= p.blocks) return;
+  idct_scaled_block<S>(p.coefs, sq, local, p.wblocks, p.dst, p.dst_stride, p.dst_w, p.dst_h);
+}
+
 }  // namespace
+
+cudaError_t launch_idct_scaled_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, int size,
+                                     cudaStream_t s) {
+  if (!ctas) return cudaSuccess;
+  count_launches(1);
+  switch (size) {
+    case 4: k_idct_scaled_batch<4><<<ctas, 128, 0, s>>>(planes, cta_end, n); break;
+    case 2: k_idct_scaled_batch<2><<<ctas, 128, 0, s>>>(planes, cta_end, n); break;
+    case 1: k_idct_scaled_batch<1><<<ctas, 128, 0, s>>>(planes, cta_end, n); break;
+    default: return cudaErrorInvalidValue;
+  }
+  return cudaGetLastError();
+}
 
 cudaError_t launch_idct_scaled(const IdctScaledParams& p, int size, cudaStream_t s) {
   if (p.nplanes < 1 || p.nplanes > 3) return cudaErrorInvalidValue;

@@ -129,6 +129,16 @@ int jpeg_scaled_geometry(const JpegFrame& f, int k, JpegScaled* g);
 // IDCT (one launch per size).  Plane c holds hblocks*s[c] rows of wblocks*s[c] samples at plane_stride[c].
 int jpeg_idct_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const d_coefs[3],
                          uint8_t* d_planes[3], int plane_stride[3]);
+// One JPEG of a batched inverse DCT: g null for the full size (jpeg_idct_dev), else jpeg_idct_scaled_dev's geometry
+struct JpegIdctJob {
+  const JpegHeader* h;
+  const JpegScaled* g;
+  int16_t* d_coefs[3];
+  uint8_t* planes[3];
+  int strides[3];
+};
+// The bytes jpeg_idct_dev / jpeg_idct_scaled_dev write for each job, with one launch per DCT scaled size for all of them
+int jpeg_idct_batch_dev(Workspace& ws, const JpegIdctJob* jobs, int n);
 // Same, coefficients decoded on the host.
 int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const h_coefs[3],
                             uint8_t* d_planes[3], int plane_stride[3]);
@@ -138,6 +148,20 @@ int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled
 // runs jpeg_host_decode_coefs, which also produces the reference's error texts.
 constexpr int kHuffDecFallback = -1000;
 int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, const JpegHeader& h, int16_t* d_coefs[3]);
+// Entropy decoding of many JPEGs at once: one relaxation over the subsequences of every scan (one host check per
+// batch of rounds for all of them), then one writing pass and one DC pass.  The coefficients are those
+// jpeg_entropy_decode_dev, or the host decoder where it declines, gives for each JPEG alone; a scan the device decoder
+// declines goes to jpeg_host_decode_coefs by itself.  Enqueued on ws.stream(), the last copies may still be in flight.
+// Returns an error only for what fails the whole batch (CUDA, memory); a corrupt scan gets its code in rc.
+struct JpegBatchScan {
+  const uint8_t* data;
+  size_t size;
+  const JpegHeader* h;
+  int16_t* d_coefs[3];  // out: [block][64] natural order, from the workspace
+  int rc;               // out: E_OK, or the error decoding this scan gives (its message in err)
+  char err[256];
+};
+int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n);
 // 0 = default = 2 = device whenever the stream allows (host only for streams the device decoder declines), 1 = host (tests, triage)
 // [0] scans decoded on the device, [1] scans handed back to the host decoder, [2] relaxation rounds of the last one
 void jpeg_entropy_decoder_stats(unsigned long long out[3]);

@@ -160,6 +160,43 @@ int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled
   return jpeg_idct_scaled_dev(ws, h, g, d_coefs, d_planes, plane_stride);
 }
 
+int jpeg_idct_batch_dev(Workspace& ws, const JpegIdctJob* jobs, int n) {
+  const size_t cap = 3 * (size_t)n;
+  for (int size = 8; size >= 1; size /= 2) {
+    IdctBatchPlane* h_pl = (IdctBatchPlane*)ws.halloc(sizeof(IdctBatchPlane) * cap);
+    unsigned* h_end = (unsigned*)ws.halloc(sizeof(unsigned) * cap);
+    if (!h_pl || !h_end) return E_MEM;
+    unsigned np = 0, ctas = 0;
+    for (int i = 0; i < n; i++) {
+      const JpegFrame& f = jobs[i].h->frame;
+      for (int c = 0; c < f.ncomp; c++) {
+        if ((jobs[i].g ? jobs[i].g->s[c] : 8) != size) continue;
+        const JpegComp& k = f.comp[c];
+        IdctBatchPlane& p = h_pl[np];
+        p.coefs = jobs[i].d_coefs[c];
+        memcpy(p.q, f.qt[k.tq], sizeof p.q);
+        p.wblocks = k.wblocks;
+        p.blocks = k.wblocks * k.hblocks;
+        p.dst = jobs[i].planes[c];
+        p.dst_stride = jobs[i].strides[c];
+        p.dst_w = size == 8 ? (k.wblocks * 8 < p.dst_stride ? k.wblocks * 8 : p.dst_stride) : k.wblocks * size;
+        p.dst_h = k.hblocks * size;
+        ctas += (unsigned)(p.blocks + 127) / 128;
+        h_end[np++] = ctas;
+      }
+    }
+    if (!np) continue;
+    IdctBatchPlane* d_pl = (IdctBatchPlane*)ws.dalloc(sizeof(IdctBatchPlane) * np);
+    unsigned* d_end = (unsigned*)ws.dalloc(sizeof(unsigned) * np);
+    if (!d_pl || !d_end) return E_MEM;
+    CUDA_TRY(cudaMemcpyAsync(d_pl, h_pl, sizeof(IdctBatchPlane) * np, cudaMemcpyHostToDevice, ws.stream()));
+    CUDA_TRY(cudaMemcpyAsync(d_end, h_end, sizeof(unsigned) * np, cudaMemcpyHostToDevice, ws.stream()));
+    if (size == 8) TIMED(ws, "idct_dequant_batch", launch_idct_dequant_batch(d_pl, d_end, np, ctas, ws.stream()));
+    else TIMED(ws, "idct_scaled_batch", launch_idct_scaled_batch(d_pl, d_end, np, ctas, size, ws.stream()));
+  }
+  return E_OK;
+}
+
 namespace {
 std::atomic<int> g_entropy_decoder{0};
 }

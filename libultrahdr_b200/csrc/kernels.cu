@@ -776,14 +776,10 @@ __device__ __forceinline__ void idct8(int d0, int d1, int d2, int d3, int d4, in
   o[4] = DESCALE(tmp13 - tmp0, shift);
 }
 
-__global__ void __launch_bounds__(128) k_idct_dequant(const IdctPlaneParams p) {
-  const int bx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int by = blockIdx.y;
-  __shared__ uint16_t sq[64];
-  if (threadIdx.x < 64) sq[threadIdx.x] = p.q[threadIdx.x];
-  __syncthreads();
-  if (bx >= p.wblocks) return;
-  const int16_t* in = p.coefs + ((size_t)by * p.wblocks + bx) * 64;
+// block (bx, by) of a plane, quantiser in shared memory
+__device__ __forceinline__ void idct_dequant_block(const int16_t* coefs, const uint16_t* sq, int wblocks, int bx, int by, uint8_t* dst,
+                                                   int dst_stride, int dst_w, int dst_h) {
+  const int16_t* in = coefs + ((size_t)by * wblocks + bx) * 64;
   int v[64];
 #pragma unroll
   for (int i = 0; i < 64; i += 8) {
@@ -808,21 +804,45 @@ __global__ void __launch_bounds__(128) k_idct_dequant(const IdctPlaneParams p) {
     idct8(v[r * 8], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3], v[r * 8 + 4], v[r * 8 + 5],
           v[r * 8 + 6], v[r * 8 + 7], o, C_BITS + P1_BITS + 3);
     const int y = by * 8 + r;
-    if (y >= p.dst_h) continue;
+    if (y >= dst_h) continue;
     unsigned lo = 0, hi = 0;
 #pragma unroll
     for (int c = 0; c < 4; c++) {
       lo |= (unsigned)min(max(o[c] + 128, 0), 255) << (8 * c);
       hi |= (unsigned)min(max(o[4 + c] + 128, 0), 255) << (8 * c);
     }
-    uint8_t* d = p.dst + (size_t)y * p.dst_stride + bx * 8;
-    if (bx * 8 + 8 <= p.dst_w && ((((size_t)d) & 7) == 0)) {
+    uint8_t* d = dst + (size_t)y * dst_stride + bx * 8;
+    if (bx * 8 + 8 <= dst_w && ((((size_t)d) & 7) == 0)) {
       *(uint2*)d = make_uint2(lo, hi);
     } else {
-      for (int c = 0; c < 8 && bx * 8 + c < p.dst_w; c++)
+      for (int c = 0; c < 8 && bx * 8 + c < dst_w; c++)
         d[c] = (uint8_t)(((c < 4 ? lo : hi) >> (8 * (c & 3))) & 0xff);
     }
   }
+}
+
+__global__ void __launch_bounds__(128) k_idct_dequant(const IdctPlaneParams p) {
+  const int bx = blockIdx.x * blockDim.x + threadIdx.x;
+  const int by = blockIdx.y;
+  __shared__ uint16_t sq[64];
+  if (threadIdx.x < 64) sq[threadIdx.x] = p.q[threadIdx.x];
+  __syncthreads();
+  if (bx >= p.wblocks) return;
+  idct_dequant_block(p.coefs, sq, p.wblocks, bx, by, p.dst, p.dst_stride, p.dst_w, p.dst_h);
+}
+
+// every plane of a batch in one launch: each CTA covers 128 blocks of one plane
+__global__ void __launch_bounds__(128) k_idct_dequant_batch(const IdctBatchPlane* __restrict__ planes, const unsigned* __restrict__ cta_end,
+                                                            unsigned n) {
+  const unsigned j = batch_find(cta_end, n, blockIdx.x);
+  const IdctBatchPlane& p = planes[j];
+  __shared__ uint16_t sq[64];
+  if (threadIdx.x < 64) sq[threadIdx.x] = p.q[threadIdx.x];
+  __syncthreads();
+  const int local = (int)(blockIdx.x - (j ? cta_end[j - 1] : 0)) * 128 + threadIdx.x;
+  if (local >= p.blocks) return;
+  const int by = local / p.wblocks, bx = local - by * p.wblocks;
+  idct_dequant_block(p.coefs, sq, p.wblocks, bx, by, p.dst, p.dst_stride, p.dst_w, p.dst_h);
 }
 
 // jdcolor.c ycc_rgb_convert with JCS_EXT_RGBA (alpha 0xFF).  ORG: a region with an origin other than 0, 0
@@ -1015,6 +1035,12 @@ cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s) {
   dim3 b(128, 1);
   dim3 g((p.wblocks + 127) / 128, p.hblocks);
   k_idct_dequant<<<g, b, 0, s>>>(p);
+  COUNT_LAUNCH();
+  return cudaGetLastError();
+}
+cudaError_t launch_idct_dequant_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s) {
+  if (!ctas) return cudaSuccess;
+  k_idct_dequant_batch<<<ctas, 128, 0, s>>>(planes, cta_end, n);
   COUNT_LAUNCH();
   return cudaGetLastError();
 }

@@ -170,6 +170,26 @@ struct IdctScaledParams {
   } plane[3];
 };
 
+// one plane of a batched inverse DCT (jpeg_idct_batch_dev): many JPEGs' planes of one DCT scaled size in one launch
+struct IdctBatchPlane {
+  const int16_t* coefs;
+  uint16_t q[64];
+  int wblocks, blocks;
+  uint8_t* dst;
+  int dst_stride;
+  int dst_w, dst_h;                 // samples beyond are not written
+};
+// first j < n with x < end[j] (end ascending): the plane of CTA x, given each plane's last CTA + 1
+__device__ __forceinline__ unsigned batch_find(const unsigned* __restrict__ end, unsigned n, unsigned x) {
+  unsigned a = 0, b = n - 1;
+  while (a < b) {
+    const unsigned m = (a + b) / 2;
+    if (x < end[m]) b = m;
+    else a = m + 1;
+  }
+  return a;
+}
+
 struct YccToRgbaParams {
   const uint8_t* y; const uint8_t* cb; const uint8_t* cr;
   int src_stride, w, h;
@@ -220,6 +240,11 @@ cudaError_t launch_resize_map(const ResizeMapParams& p, cudaStream_t s);
 cudaError_t launch_fdct8(const Fdct8Params& p, cudaStream_t s);
 cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s);
 cudaError_t launch_idct_scaled(const IdctScaledParams& p, int size, cudaStream_t s);
+// planes / cta_end: n entries in device memory, cta_end the inclusive prefix of the planes' ceil(blocks / 128) CTAs,
+// `ctas` its last entry.  size 8: k_idct_dequant's arithmetic, 4 / 2 / 1: k_idct_scaled's.
+cudaError_t launch_idct_dequant_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s);
+cudaError_t launch_idct_scaled_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, int size,
+                                     cudaStream_t s);
 cudaError_t launch_ycc_to_rgba(const YccToRgbaParams& p, cudaStream_t s);
 
 // number of kernel launches issued by this library since load (bench.py's gpu_launches)

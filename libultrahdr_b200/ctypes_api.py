@@ -85,6 +85,19 @@ def declare_scaled_decode(lib):
     return lib
 
 
+class DecodeItem(C.Structure):
+    """uhdr_b200_decode_item_t: one file of uhdr_b200_decode_batch_dev"""
+    _fields_ = [("data", C.c_void_p), ("size", C.c_size_t), ("dest_dev", C.POINTER(RawImage)),
+                ("gainmap_dev", C.POINTER(RawImage)), ("metadata_out", C.POINTER(GainmapMetadata)),
+                ("status", C.c_int)]
+
+
+def declare_decode_batch(lib):
+    """argument types of uhdr_b200_decode_batch_dev (include/uhdr_b200.h) on a loaded libuhdr_b200"""
+    lib.uhdr_b200_decode_batch_dev.argtypes = [C.POINTER(DecodeItem), C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
+    return lib
+
+
 def declare_resident_image(lib):
     """argument types of the device-resident image entry points (uhdr_b200_image_*, include/uhdr_b200.h)"""
     lib.uhdr_b200_image_open_dev.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]
