@@ -220,6 +220,36 @@ UHDR_EXTERN int uhdr_b200_encode_dev(const uhdr_raw_image_t* hdr_dev, const uhdr
 UHDR_EXTERN int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img_dev, int quality, const void* icc,
                                           size_t icc_size, void* out, size_t cap, size_t* out_size, void* stream);
 
+/* Transcoding: a smaller or recompressed JPEG/R made from a JPEG/R, keeping its SDR rendition and its gain map (no
+ * decode to HDR pixels, no new tone mapping).  Both JPEGs of the file are decoded at 1/k, as libjpeg-turbo decodes
+ * with scale_denom = k (raw YCbCr planes, the 3-channel map too), re-encoded, and put into a new container with the
+ * file's metadata.  The output bytes equal this composition of the reference's pieces:
+ *  - each JPEG's planes, as JpegDecoderHelper's raw_data_out decode at 1/k gives them (tight strides), re-encoded by
+ *    JpegEncoderHelper::compressImage in the format they form (Y400, YUV420, YUV422 or YUV444) at base_quality /
+ *    gainmap_quality, with that JPEG's own ICC APP2 payload (none if it has none);
+ *  - base_420 = 1 and a 4:4:4 base (a 4:4:4 file, or a 4:2:0 one at k > 1): the base is instead what libjpeg-turbo's
+ *    jpeg_write_scanlines writes from the YCbCr planes with 2x2 / 1x1 / 1x1 sampling -- libjpeg's own chroma
+ *    downsampling, (a + b + c + d + bias) >> 2 with bias 1, 2, 1, 2, ... along a row, edges replicated.  A base that
+ *    is already 4:2:0 is taken as above, a gray base ignores the flag, 4:2:2 gives UHDR_CODEC_UNSUPPORTED_FEATURE;
+ *  - keep_exif = 1: the primary image's EXIF block is carried into the new file;
+ *  - the container is what API-4 (uhdr_enc_set_compressed_image with the primary image's ICC gamut,
+ *    uhdr_enc_set_gainmap_image with the file's metadata, uhdr_encode) writes: ISO 21496-1 metadata, MPF, ICC.
+ * Input and output are HOST bytes; the work runs on the calling thread's codec for the current device and the call
+ * returns when the file is complete.  Errors: those of the composition (corrupt or progressive data, no metadata,
+ * 4:2:2 / 4:4:0 / 4:1:1 at k > 1 as uhdr_b200_decode_scaled_dev, a sampling the encoder does not write, API-4's
+ * checks); a k outside {1, 2, 4, 8}, a quality outside 0..100 or a null pointer give UHDR_CODEC_INVALID_PARAM.  A cap
+ * that is too small gives UHDR_CODEC_MEM_ERROR with *out_size set to the size needed.  Nothing is written to out on
+ * failure.  Without a device: UHDR_CODEC_ERROR with a CUDA message.  New fields go at the end of the struct. */
+typedef struct uhdr_b200_transcode_config {
+  int k;               /* 1, 2, 4 or 8: both JPEGs reduced as libjpeg-turbo's scale_denom = k does */
+  int base_quality;    /* 0..100 */
+  int gainmap_quality; /* 0..100 */
+  int base_420;        /* 0: the base keeps the sampling its scaled decode produced; 1: the base is written 4:2:0 */
+  int keep_exif;       /* 1: the primary image's EXIF block is carried into the new file */
+} uhdr_b200_transcode_config_t;
+UHDR_EXTERN int uhdr_b200_transcode(const void* data, size_t size, const uhdr_b200_transcode_config_t* cfg, void* out,
+                                    size_t cap, size_t* out_size);
+
 /* Measurement hooks.  Kernel timing brackets every kernel launch with CUDA events on the
  * launching stream and accumulates per-kernel totals ("name count total_ms min_ms max_ms" lines).
  * uhdr_b200_enc_rearm() makes a finished encoder handle runnable again while keeping the inputs

@@ -565,6 +565,22 @@ UHDR_API int uhdr_b200_encode_dev(const uhdr_raw_image_t* hdr, const uhdr_raw_im
   return rc;
 }
 
+UHDR_API int uhdr_b200_transcode(const void* data, size_t size, const uhdr_b200_transcode_config_t* cfg, void* out, size_t cap,
+                                 size_t* out_size) {
+  if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed img->data field");
+  if (!cfg) return fail(E_INVALID_PARAM, "received nullptr for the transcode configuration");
+  int rc = check_out(out, out_size);
+  if (rc) return rc;
+  if (!valid_scale(cfg->k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", cfg->k);
+  if (cfg->base_quality < 0 || cfg->base_quality > 100 || cfg->gainmap_quality < 0 || cfg->gainmap_quality > 100)
+    return fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", cfg->base_quality, cfg->gainmap_quality);
+  DecodedInfo info;
+  if ((rc = JpegRCodec().probe((const uint8_t*)data, size, &info))) return rc;  // host only
+  JpegRCodec* c = nullptr;
+  if ((rc = dev_codec(&c))) return rc;
+  return c->transcode((const uint8_t*)data, size, info, *cfg, (uint8_t*)out, cap, out_size);
+}
+
 UHDR_API int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img, int quality, const void* icc, size_t icc_size, void* out,
                                        size_t cap, size_t* out_size, void* stream) {
   if (!img) return fail(E_INVALID_PARAM, "received nullptr argument");

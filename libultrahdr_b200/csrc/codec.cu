@@ -11,8 +11,6 @@
 
 namespace uhdr_b200 {
 
-static ByteView find_marker(const uint8_t* d, const JpegHeader& h, uint8_t id, const char* sig, size_t sig_len);
-
 // ------------------------------------------------------------------------------------------------
 // encode
 // ------------------------------------------------------------------------------------------------
@@ -60,7 +58,7 @@ static int block_stage_input(Workspace& ws, DevImage* img) {
 //    row (0 / 128, the block stage's fill)
 // `img` holds the workspace copy of `caller` (zero-tailed); this rebuilds the helper's bytes in it.  rows[c] = rows
 // of plane c the block stage reads from memory (0: up to the height, then the fill).
-static int helper_padding(Workspace& ws, const uhdr_raw_image_t& caller, cudaMemcpyKind kind, const DevImage& img, int rows[3]) {
+int helper_padding(Workspace& ws, const uhdr_raw_image_t& caller, cudaMemcpyKind kind, const DevImage& img, int rows[3]) {
   if (img.v.fmt != F_Y400 && img.v.fmt != F_YUV420 && img.v.fmt != F_YUV422 && img.v.fmt != F_YUV444) return E_OK;
   cudaStream_t st = ws.stream();
   for (int i = 0; i < fmt_planes(img.v.fmt); i++) {
@@ -346,7 +344,7 @@ static int validate_header(const JpegHeader& h) {  // jpegdecoderhelper.cpp:244-
 }
 
 // first marker `id` whose payload starts with `sig`, as a view into the stream (jpegdecoderhelper.cpp:119-139 copies it)
-static ByteView find_marker(const uint8_t* d, const JpegHeader& h, uint8_t id, const char* sig, size_t sig_len) {
+ByteView find_marker(const uint8_t* d, const JpegHeader& h, uint8_t id, const char* sig, size_t sig_len) {
   ByteView v;
   for (const JpegMarker& m : h.markers)
     if (m.id == id && m.length > sig_len && !memcmp(d + m.offset, sig, sig_len)) {
@@ -580,7 +578,7 @@ int JpegRCodec::decode(const uint8_t* data, size_t size, int out_ct, int out_fmt
 
 int JpegRCodec::decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go, size_t gl, int sdr_mode,
                             YccToRgbaParams* to_rgba, bool want_map, int k, DevImage* sdr, DevImage* map, JpegHeader* ph,
-                            JpegHeader* gh, PhaseTrace& tr) {
+                            JpegHeader* gh, PhaseTrace& tr, int map_mode) {
   int rc = E_OK;
   // both images sizeable: the gain-map JPEG goes to a helper thread with its own stream
   const bool overlap = want_map && pl >= (256u << 10) && gl >= (256u << 10);
@@ -590,9 +588,9 @@ int JpegRCodec::decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go
     size_t len;
     DevImage* map;
     JpegHeader* gh;
-    int dev, k, rc;
+    int dev, k, mode, rc;
     char err[256];
-  } mj{this, data + go, gl, map, gh, 0, k, E_OK, {0}};
+  } mj{this, data + go, gl, map, gh, 0, k, map_mode, E_OK, {0}};
   if (overlap) {
     if (!ws2_) {
       ws2_.reset(new Workspace());
@@ -606,7 +604,7 @@ int JpegRCodec::decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go
       MapJob& j = *static_cast<MapJob*>(a);
       auto fail_with = [&](int rc, const char* what) { j.rc = rc; snprintf(j.err, sizeof j.err, "%s", what); };
       if (cudaSetDevice(j.dev) != cudaSuccess) return fail_with(E_ERROR, "cudaSetDevice failed in the gain-map decode thread");
-      j.rc = j.self->decode_jpeg_dev(*j.self->ws2_, j.data, j.len, 2, j.map, j.gh, nullptr, j.k);  // DECODE_STREAM :1486
+      j.rc = j.self->decode_jpeg_dev(*j.self->ws2_, j.data, j.len, j.mode, j.map, j.gh, nullptr, j.k);
       if (j.rc) snprintf(j.err, sizeof j.err, "%s", last_error());
       else if (cudaEventRecord(j.self->map_ready_, j.self->ws2_->stream()) != cudaSuccess) fail_with(E_ERROR, "cudaEventRecord failed");
     }, &mj);
@@ -623,7 +621,7 @@ int JpegRCodec::decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go
       CUDA_TRY(cudaStreamWaitEvent(ws_.stream(), map_ready_, 0));
       if (kernel_timing_enabled()) ws2_->sync();
     } else {
-      rc = decode_jpeg_dev(ws_, data + go, gl, 2, map, gh, nullptr, k);  // DECODE_STREAM :1486
+      rc = decode_jpeg_dev(ws_, data + go, gl, map_mode, map, gh, nullptr, k);
       if (rc) return rc;
     }
     blob = find_marker(data + go, *gh, 0xE2, "ICC_PROFILE", 12);

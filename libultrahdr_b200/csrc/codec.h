@@ -139,6 +139,11 @@ class JpegRCodec {
   int decode_jpeg_dev(const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* hdr, int k = 1) {
     return decode_jpeg_dev(ws_, data, size, mode, out, hdr, nullptr, k);
   }
+  // uhdr_b200_transcode (transcode.cu): both JPEGs of the file decoded at 1/cfg.k as raw planes, re-encoded at the
+  // configured qualities -- the base image optionally 4:2:0 through libjpeg's scanline downsampling -- and assembled
+  // as API-4 assembles them, with the file's ICC profiles, metadata and (keep_exif) EXIF.  `probed`: probe() of data.
+  int transcode(const uint8_t* data, size_t size, const DecodedInfo& probed, const uhdr_b200_transcode_config_t& cfg,
+                uint8_t* out, size_t cap, size_t* out_size);
   ~JpegRCodec();
 
  private:
@@ -148,9 +153,11 @@ class JpegRCodec {
                       YccToRgbaParams* to_rgba = nullptr, int k = 1);
   // both JPEGs of a JPEG/R (po / pl, go / gl: their spans in data) on this codec's streams -- the gain map's on the
   // helper thread when both are sizeable, joined into ws_ -- and the gamuts of their ICC profiles; want_map false: the
-  // primary only.  sdr_mode / to_rgba: decode_jpeg_dev's mode / to_rgba of the primary.
+  // primary only.  sdr_mode / to_rgba: decode_jpeg_dev's mode / to_rgba of the primary; map_mode: the map's mode
+  // (2 = DECODE_STREAM, what decodeJPEGR uses, jpegr.cpp:1486).
   int decode_pair(const uint8_t* data, size_t po, size_t pl, size_t go, size_t gl, int sdr_mode, YccToRgbaParams* to_rgba,
-                  bool want_map, int k, DevImage* sdr, DevImage* map, JpegHeader* ph, JpegHeader* gh, PhaseTrace& tr);
+                  bool want_map, int k, DevImage* sdr, DevImage* map, JpegHeader* ph, JpegHeader* gh, PhaseTrace& tr,
+                  int map_mode = 2);
   int decode_body(const uint8_t* data, size_t size, int out_ct, int out_fmt, float max_display_boost,
                   uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out, uhdr_gainmap_metadata_t* md_out,
                   const DecodedInfo* probed, const cudaStream_t* dev_stream, int k, const DecodeEffects* fx);
@@ -191,6 +198,12 @@ int compress_image_dev(Workspace& ws, const DevImage& img, int quality, const vo
 // C++ JpegEncoderHelper): upload_image, then the helper's edge padding of planes whose width is not a multiple of 8
 // for the caller's strides (jpegencoderhelper.cpp:246-309).  rows[c] goes to jpeg_forward_dev.
 int upload_jpeg_input(Workspace& ws, const uhdr_raw_image_t& src, DevImage* out, int rows[3]);
+// upload_jpeg_input's second half: the helper's padding of `img`, a workspace copy of `caller`'s planes made with
+// upload_image (kind: where caller's planes are)
+int helper_padding(Workspace& ws, const uhdr_raw_image_t& caller, cudaMemcpyKind kind, const DevImage& img, int rows[3]);
+
+// first APPn marker `id` of a header whose payload starts with `sig`, as a view into the stream d
+ByteView find_marker(const uint8_t* d, const JpegHeader& h, uint8_t id, const char* sig, size_t sig_len);
 
 // uhdr_enc_set_raw_image's checks of one intent's descriptor (ultrahdr_api.cpp:842-1025): its code, the last error
 // set.  The planes are not dereferenced.

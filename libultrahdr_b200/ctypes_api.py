@@ -19,6 +19,7 @@ HDR_IMG, SDR_IMG, BASE_IMG, GAIN_MAP_IMG = 0, 1, 2, 3
 # uhdr_enc_preset_t
 USAGE_REALTIME, USAGE_BEST_QUALITY = 0, 1
 CODEC_OK = 0
+CODEC_ERROR, CODEC_INVALID_PARAM, CODEC_MEM_ERROR, CODEC_UNSUPPORTED = 1, 3, 4, 6
 
 FLT_MAX = float(np.finfo(np.float32).max)
 FLT_MIN = float(np.finfo(np.float32).tiny)
@@ -152,3 +153,16 @@ def yuv420_image(buf, w, h, cg, ct=CT_SRGB, rng=CR_FULL):
     v = buf[w * h + (w // 2) * (h // 2):]
     img = raw_image(FMT_YUV420, cg, ct, rng, w, h, [y, u, v], [w, w // 2, w // 2])
     return img, (y, u, v)
+
+
+class TranscodeConfig(C.Structure):
+    """uhdr_b200_transcode_config_t"""
+    _fields_ = [("k", C.c_int), ("base_quality", C.c_int), ("gainmap_quality", C.c_int), ("base_420", C.c_int),
+                ("keep_exif", C.c_int)]
+
+
+def declare_transcode(lib):
+    """argument types of uhdr_b200_transcode (include/uhdr_b200.h) on a loaded libuhdr_b200"""
+    lib.uhdr_b200_transcode.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(TranscodeConfig), C.c_void_p, C.c_size_t,
+                                        C.POINTER(C.c_size_t)]
+    return lib
