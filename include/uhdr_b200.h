@@ -249,6 +249,34 @@ typedef struct uhdr_b200_transcode_config {
 } uhdr_b200_transcode_config_t;
 UHDR_EXTERN int uhdr_b200_transcode(const void* data, size_t size, const uhdr_b200_transcode_config_t* cfg, void* out,
                                     size_t cap, size_t* out_size);
+/* uhdr_b200_transcode of many files in one call, for thumbnail and preview jobs over many uploads: both JPEGs of every
+ * file go through one entropy decoding, one inverse DCT per reduced size, one staging pass, one block stage and one
+ * entropy coding, with two host waits for the encoder, instead of a single call's fixed cost per file.
+ *  - Each item gets exactly what uhdr_b200_transcode(data, size, cfg, out, cap, &out_size) gives for that file alone:
+ *    the same bytes, out_size and status.  One cfg (k, both qualities, base_420, keep_exif) applies to every item.
+ *  - A failing item gets the code the single call returns and nothing is written to its out (corrupt or progressive
+ *    data, no metadata, 4:2:2 at k > 1 or with base_420, API-4's checks, a short cap: UHDR_CODEC_MEM_ERROR with
+ *    out_size set to the size needed).  The others are unaffected.  The return value is UHDR_CODEC_OK when every item
+ *    succeeded, else the first failing item's code, and uhdr_b200_last_error() names that item's index and gives its
+ *    message.  An error of the whole call (CUDA, device memory) is returned and set as the status of every item without
+ *    an error of its own.
+ *  - A null items or cfg, n < 1, a k outside {1, 2, 4, 8} or a quality outside 0..100 give UHDR_CODEC_INVALID_PARAM
+ *    and transcode nothing.  Without a device: UHDR_CODEC_ERROR with a CUDA message.
+ *  - Input and output are HOST bytes; the call returns when every file is complete.  It runs on the calling thread's
+ *    codec for the current device, as uhdr_b200_transcode does, and the two may be interleaved on one thread.
+ *  - A batch whose scratch would exceed a device-memory budget (4 GiB; the environment variable
+ *    UHDR_B200_BATCH_GROUP_BYTES sets another) is transcoded in groups, one after the other, with the same results.
+ *  - A repeated batch of the same or a smaller size makes no heap call. */
+typedef struct uhdr_b200_transcode_item {
+  const void* data;  /* one JPEG/R file, host memory */
+  size_t size;
+  void* out;         /* host buffer for the new file */
+  size_t cap;
+  size_t out_size;   /* out: bytes written; with UHDR_CODEC_MEM_ERROR, the size needed */
+  int status;        /* out: this item's uhdr_codec_err_t */
+} uhdr_b200_transcode_item_t;
+UHDR_EXTERN int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n,
+                                          const uhdr_b200_transcode_config_t* cfg);
 
 /* Measurement hooks.  Kernel timing brackets every kernel launch with CUDA events on the
  * launching stream and accumulates per-kernel totals ("name count total_ms min_ms max_ms" lines).
@@ -295,6 +323,10 @@ UHDR_EXTERN void uhdr_b200_apply_stats(unsigned long long out[4]);
  * since process start, every entry point: out[0] = resident CTAs per wave the plan assumed (0 before the first
  * encode), out[1..8] = launches with bpt = 1..8, out[9] = launches whose grid exceeded one wave.  Host-side counts. */
 UHDR_EXTERN void uhdr_b200_jpeg_encode_stats(unsigned long long out[10]);
+/* The batched entropy coder (k_huff_encode_batch, uhdr_b200_transcode_batch: one launch per group of items, bpt chosen by
+ * the rule above over all the group's blocks; not counted in uhdr_b200_jpeg_encode_stats).  Since process start:
+ * out[0] = launches, out[1] = scans they coded.  Host-side counts. */
+UHDR_EXTERN void uhdr_b200_jpeg_encode_batch_stats(unsigned long long out[2]);
 /* diagnostic: worst[0] = max |approximate pow(e, 1/2.4) - the exact one| over the `count` floats whose bit patterns
  * start at first_bits (the screen relies on <= 3e-7 for e in (0.0031308, 1]; must measure <= 1.5e-7); host pointer. */
 UHDR_EXTERN int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst);

@@ -87,6 +87,10 @@ UHDR_API void uhdr_b200_jpeg_encode_stats(unsigned long long out[10]) {
   if (out) jpeg_encode_stats(out);
 }
 
+UHDR_API void uhdr_b200_jpeg_encode_batch_stats(unsigned long long out[2]) {
+  if (out) jpeg_encode_batch_stats(out);
+}
+
 UHDR_API int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst) {
   Workspace* ws = tls_workspace();
   if (!ws || !worst) return E_ERROR;
@@ -579,6 +583,54 @@ UHDR_API int uhdr_b200_transcode(const void* data, size_t size, const uhdr_b200_
   JpegRCodec* c = nullptr;
   if ((rc = dev_codec(&c))) return rc;
   return c->transcode((const uint8_t*)data, size, info, *cfg, (uint8_t*)out, cap, out_size);
+}
+
+UHDR_API int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n, const uhdr_b200_transcode_config_t* cfg) {
+  // uhdr_b200_transcode's call-level checks, before any device work
+  if (!items) return fail(E_INVALID_PARAM, "received nullptr for the items");
+  if (n < 1) return fail(E_INVALID_PARAM, "received %d items, expects at least 1", n);
+  if (!cfg) return fail(E_INVALID_PARAM, "received nullptr for the transcode configuration");
+  if (!valid_scale(cfg->k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", cfg->k);
+  if (cfg->base_quality < 0 || cfg->base_quality > 100 || cfg->gainmap_quality < 0 || cfg->gainmap_quality > 100)
+    return fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", cfg->base_quality, cfg->gainmap_quality);
+  static thread_local std::vector<TranscodeBatchItem> its;  // grow-only: a batch of the same or a smaller size takes no heap
+  if ((int)its.size() < n) its.resize(n);
+  for (int i = 0; i < n; i++) {
+    const uhdr_b200_transcode_item_t& in = items[i];
+    TranscodeBatchItem& b = its[i];
+    b.data = (const uint8_t*)in.data;
+    b.size = in.size;
+    b.out = (uint8_t*)in.out;
+    b.cap = in.cap;
+    b.out_size = 0;
+    // uhdr_b200_transcode's per-file checks, in its order
+    b.rc = !in.data ? fail(E_INVALID_PARAM, "received nullptr for compressed img->data field")
+                    : !in.out ? fail(E_INVALID_PARAM, "received nullptr for the output buffer")
+                              : JpegRCodec().probe(b.data, b.size, &b.info);   // host only
+    if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
+  }
+  JpegRCodec* c = nullptr;
+  int rc = dev_codec(&c);
+  if (!rc) {
+    size_t group = size_t(4) << 30;
+    if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
+    rc = c->transcode_batch(its.data(), n, *cfg, group);
+  }
+  std::string call_err = rc ? last_error() : "";
+  int first = -1;
+  for (int i = 0; i < n; i++) {
+    TranscodeBatchItem& b = its[i];
+    if (rc && !b.rc) {  // an error of the whole call: every item without its own
+      b.rc = rc;
+      snprintf(b.err, sizeof b.err, "%s", call_err.c_str());
+    }
+    items[i].status = b.rc;
+    // out_size: bytes written, or with UHDR_CODEC_MEM_ERROR the size needed (0 when the file was not assembled)
+    items[i].out_size = !b.rc || b.rc == E_MEM ? b.out_size : 0;
+    if (b.rc && first < 0) first = i;
+  }
+  if (first < 0) return E_OK;
+  return fail(its[first].rc, "item %d: %s", first, its[first].err);
 }
 
 UHDR_API int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img, int quality, const void* icc, size_t icc_size, void* out,

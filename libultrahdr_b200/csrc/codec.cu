@@ -399,8 +399,7 @@ JpegRCodec::~JpegRCodec() {
   if (writes_done_) cudaEventDestroy(writes_done_);
 }
 
-// decode_jpeg_dev up to the entropy decoding: the header, its checks, the output planes
-static int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, int mode, int k, DevImage* out, JpegHeader* h,
+int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, int mode, int k, DevImage* out, JpegHeader* h,
                              JpegDecodeJob* j) {
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed image data");
   if (size == 0) return fail(E_INVALID_PARAM, "received bad compressed image size %zd", size);
@@ -443,8 +442,7 @@ static int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, in
   return E_OK;
 }
 
-// decode_jpeg_dev after the inverse DCT: the colour conversion (mode 1) or the planes' format (mode 0)
-static int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, DevImage* out, YccToRgbaParams* to_rgba) {
+int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, DevImage* out, YccToRgbaParams* to_rgba) {
   const JpegFrame& f = h->frame;
   const int mode = j.mode;
   const bool scaled = j.k != 1;
@@ -854,26 +852,14 @@ static void batch_item_fail(DecodeBatchItem& it, int rc, const char* msg) {
 
 int JpegRCodec::decode_batch(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller,
                              size_t group_bytes) {
-  int rc = E_OK;
-  for (int g0 = 0; g0 < n && !rc;) {
-    // a group: as many items as fit the scratch budget (at least one); the entropy-coded bytes of a group stay below
-    // 2^29 so that every bit position of the group fits 32 bits
-    size_t bytes = 0, coded = 0;
-    int g1 = g0;
-    for (; g1 < n; g1++) {
-      const DecodedInfo& in = items[g1].info;
-      // coefficients (128 B per 8x8 block, at most 3 components at full size) and their DC terms, planes, coded bits
-      const size_t px = (size_t)in.width * k * in.height * k + (size_t)in.gm_width * k * in.gm_height * k;
-      const size_t b = px * 7 + (size_t)(in.width * in.height + in.gm_width * in.gm_height) * 16 + 2 * items[g1].size;
-      if (g1 > g0 && (bytes + b > group_bytes || coded + items[g1].size >= (1u << 29))) break;
-      bytes += b;
-      coded += items[g1].size;
-    }
-    if (g0 > 0 && (rc = ws_.sync())) break;  // the previous group's pinned staging is rewound below
-    ws_.rewind();
-    rc = decode_batch_group(items + g0, g1 - g0, k, out_ct, max_display_boost, caller);
-    g0 = g1;
-  }
+  auto cost = [&](int i, size_t* coded) {
+    const DecodedInfo& in = items[i].info;   // at 1/k
+    *coded = items[i].size;
+    return batch_decode_bytes(in.width, in.height, in.gm_width, in.gm_height, k, items[i].size);
+  };
+  const int rc = for_each_group(n, group_bytes, cost, [&](int g0, int g1) {
+    return decode_batch_group(items + g0, g1 - g0, k, out_ct, max_display_boost, caller);
+  });
   if (int r = mark_in_flight()) return rc ? rc : r;
   if (rc) return rc;
   CUDA_TRY(cudaStreamWaitEvent(caller, writes_done_, 0));

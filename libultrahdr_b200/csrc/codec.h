@@ -50,6 +50,31 @@ struct DecodeBatchItem {
   char map_err[256] = {0};
 };
 
+// One file of JpegRCodec::transcode_batch.  The caller fills the first group of fields; rc != E_OK on entry skips the item.
+struct TranscodeBatchItem {
+  const uint8_t* data = nullptr;
+  size_t size = 0;
+  DecodedInfo info;  // probe() of the file
+  uint8_t* out = nullptr;
+  size_t cap = 0;
+  size_t out_size = 0;  // out: what transcode() sets
+  int rc = 0;        // out: the code transcode() gives for this file alone, its message in err
+  char err[256] = {0};
+  // the transcode's state between its batched stages
+  JpegHeader ph, gh;
+  JpegDecodeJob pj, gj;
+  DevImage sdr{}, map{};
+  int map_rc = 0;    // an error of the gain-map JPEG's header stage, returned after the primary image's own
+  char map_err[256] = {0};
+  JpegEncodeJob base_jpeg, gm_jpeg;
+};
+
+// decode_jpeg_dev's stages (codec.cu): up to the entropy decoding (the header, its checks, the output planes), and after
+// the inverse DCT (the colour conversion of mode 1, or the planes' format of mode 0)
+int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, int mode, int k, DevImage* out, JpegHeader* h,
+                      JpegDecodeJob* j);
+int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, DevImage* out, YccToRgbaParams* to_rgba);
+
 // One parked host thread per codec (spawned on first use, kept until the codec dies): runs the gain-map JPEG of a
 // decode next to the primary one without creating a thread per call.
 class ParkedThread {
@@ -144,6 +169,11 @@ class JpegRCodec {
   // as API-4 assembles them, with the file's ICC profiles, metadata and (keep_exif) EXIF.  `probed`: probe() of data.
   int transcode(const uint8_t* data, size_t size, const DecodedInfo& probed, const uhdr_b200_transcode_config_t& cfg,
                 uint8_t* out, size_t cap, size_t* out_size);
+  // transcode() of many files with one entropy decoding, one inverse DCT, one staging launch, one block-stage launch and
+  // one entropy-coding launch per group of items (groups as decode_batch forms them, the encoder's scratch included),
+  // and two host waits for the encoder.  Each item gets the bytes, size and code transcode() gives for it alone; a
+  // failing item writes nothing.  The return value is an error that ends the whole call (CUDA, memory).
+  int transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg, size_t group_bytes);
   ~JpegRCodec();
 
  private:
@@ -174,8 +204,40 @@ class JpegRCodec {
                          const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                          uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out);
   int decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller);
-  std::vector<JpegBatchScan> batch_scans_;   // grow-only scratch of decode_batch
+  int transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg);
+  // transcode()'s last stage, once both scans are on the host: API-4's checks, the heads, EXIF, the container, the cap
+  int transcode_finish(const uint8_t* data, const DecodedInfo& probed, const JpegHeader& ph, const JpegHeader& gh,
+                       const JpegEncodeJob& base_jpeg, const JpegEncodeJob& gm_jpeg, const uhdr_b200_transcode_config_t& cfg,
+                       uint8_t* out, size_t cap, size_t* out_size);
+  static int fail_base_422();
+  // scratch of one file of a batched decode at 1/k (w x h, gw x gh: the 1/k sizes; size: the file's bytes)
+  static size_t batch_decode_bytes(int w, int h, int gw, int gh, int k, size_t size);
+  // The batches' groups: items [g0, g1) as long as their scratch cost(i, &coded) fits `group_bytes` (at least one item)
+  // and their entropy-coded bytes stay below 2^29, so that every bit position of a group fits 32 bits.  run(g0, g1)
+  // runs each group once the previous one's work is done on the host and the workspace is rewound.
+  template <class Cost, class Run>
+  int for_each_group(int n, size_t group_bytes, Cost cost, Run run) {
+    int rc = E_OK;
+    for (int g0 = 0; g0 < n && !rc;) {
+      size_t bytes = 0, coded = 0;
+      int g1 = g0;
+      for (; g1 < n; g1++) {
+        size_t c = 0;
+        const size_t b = cost(g1, &c);
+        if (g1 > g0 && (bytes + b > group_bytes || coded + c >= (1u << 29))) break;
+        bytes += b;
+        coded += c;
+      }
+      if (g0 > 0 && (rc = ws_.sync())) break;  // the previous group's pinned staging is rewound below
+      ws_.rewind();
+      rc = run(g0, g1);
+      g0 = g1;
+    }
+    return rc;
+  }
+  std::vector<JpegBatchScan> batch_scans_;   // grow-only scratch of decode_batch and transcode_batch
   std::vector<JpegIdctJob> batch_idct_;
+  std::vector<JpegEncodeJob*> batch_enc_;
   Workspace ws_;
   // second stream + arenas: the gain-map JPEG of a decode is processed by a helper thread while the
   // calling thread handles the primary image (both entropy decoders alternate host and device phases)

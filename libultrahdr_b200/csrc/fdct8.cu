@@ -374,6 +374,66 @@ __global__ void __launch_bounds__(256, 4) k_fdct8_code(const __grid_constant__ F
   }
 }
 
+// k_fdct8_code over the planes of many images (no RGB888): a warp item is 32 consecutive blocks of one plane, found by a
+// binary search over the planes' cumulative item counts; a plane's tq[0] picks one of four quantisers (base luma,
+// base chroma, map luma, map chroma)
+struct Fdct8BatchParams {
+  const Fdct8Plane* planes;
+  const unsigned* item_end;   // cumulative warp items of the planes
+  unsigned nplanes, total;
+  uint16_t q[4][64];
+  unsigned mag[4][64];
+  const uint32_t* acbooks;
+};
+struct CodeBatchSmem {
+  unsigned sdiv[4][64], smag[4][64];
+  uint32_t acb[2][256];
+  int tiles[8][4 * kTileStride];
+  alignas(16) int16_t stage[8][32 * kStagePitch];
+  uint8_t unzig[64];
+};
+
+__global__ void __launch_bounds__(256, 4) k_fdct8_code_batch(const __grid_constant__ Fdct8BatchParams P) {
+  extern __shared__ uint4 smem_u4[];
+  CodeBatchSmem& S = *reinterpret_cast<CodeBatchSmem*>(smem_u4);
+  S.acb[0][threadIdx.x] = __ldg(P.acbooks + threadIdx.x);
+  S.acb[1][threadIdx.x] = __ldg(P.acbooks + 256 + threadIdx.x);
+  if (threadIdx.x < 64) S.unzig[threadIdx.x] = (uint8_t)unzig_rt(threadIdx.x);
+  {
+    const int t = threadIdx.x >> 6, i = threadIdx.x & 63;
+    S.sdiv[t][i] = (unsigned)P.q[t][i] << 3;
+    S.smag[t][i] = P.mag[t][i];
+  }
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane_b = lane >> 3, lane_r = lane & 7;
+  int* tile = S.tiles[warp];
+  int16_t* stage = S.stage[warp];
+#pragma unroll 1
+  for (unsigned it = blockIdx.x * 8 + warp; it < P.total; it += gridDim.x * 8) {
+    const unsigned pi = batch_find(P.item_end, P.nplanes, it);
+    const Fdct8Plane& pl = P.planes[pi];
+    const int local = (int)(it - (pi ? P.item_end[pi - 1] : 0u));
+    const int nb = pl.wblocks * pl.hblocks;
+    const int tq = pl.tq[0];
+    const int base = local * 32;
+    int d[8];
+#pragma unroll 1
+    for (int s = 0; s < 8; s++) {
+      const int f = min(base + s * 4 + lane_b, nb - 1);   // past the end: a valid block, nothing stored later
+      const int by = f / pl.wblocks, bx = f - by * pl.wblocks;
+      load_plane_row(pl, by, bx, lane_r, d);
+      block_to_stage(d, tile, lane_b, lane_r, S.sdiv[tq], S.smag[tq], S.unzig, stage + (s * 4 + lane_b) * kStagePitch);
+    }
+    __syncwarp();
+    const int f = base + lane;
+    const bool live = f < nb;
+    code_block_lane(stage + lane * kStagePitch, S.acb[pl.hsel[0]], live ? reinterpret_cast<uint32_t*>(pl.coefs[0] + (size_t)f * 128) : nullptr,
+                    live ? pl.meta[0] + f : nullptr);
+    __syncwarp();
+  }
+}
+
 }  // namespace
 
 void jpeg_std_codebook(int which, uint32_t out[256]);  // jpeg_host.cpp: (code << 8 | length) per symbol
@@ -452,6 +512,40 @@ cudaError_t launch_fdct8(const Fdct8Params& Pin, cudaStream_t s) {
     const int ctas = total < resident ? total : resident;
     k_fdct8<false><<<ctas, 256, 0, s>>>(P);
   }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_fdct8_code_batch(const Fdct8Plane* planes, const unsigned* item_end, unsigned nplanes, unsigned total_items,
+                                    const uint16_t q[4][64], cudaStream_t s) {
+  if (!total_items) return cudaSuccess;
+  count_launches(1);
+  Fdct8BatchParams P;
+  memset(&P, 0, sizeof P);
+  P.planes = planes;
+  P.item_end = item_end;
+  P.nplanes = nplanes;
+  P.total = total_items;
+  if (fdct_device_books(&P.acbooks)) return cudaErrorUnknown;
+  for (int t = 0; t < 4; t++)
+    for (int i = 0; i < 64; i++) {
+      P.q[t][i] = q[t][i];
+      const unsigned d = (unsigned)q[t][i] << 3;
+      P.mag[t][i] = d ? (unsigned)((0x100000000ull + d - 1) / d) : 0u;
+    }
+  static int resident = 0;  // CTAs of one wave
+  if (!resident) {
+    int per_sm = 0, dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaFuncSetAttribute(k_fdct8_code_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CodeBatchSmem));
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fdct8_code_batch, 256, sizeof(CodeBatchSmem)) != cudaSuccess ||
+        per_sm < 1)
+      per_sm = 1;
+    resident = per_sm * (sms > 0 ? sms : 132);
+  }
+  const unsigned need = (total_items + 7) / 8;
+  const unsigned ctas = need < (unsigned)resident ? need : (unsigned)resident;
+  k_fdct8_code_batch<<<ctas, 256, sizeof(CodeBatchSmem), s>>>(P);
   return cudaGetLastError();
 }
 

@@ -59,10 +59,21 @@ struct JpegEncodeJob {
 // not only those up to the plane height
 int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag = false,
                      const int* rows = nullptr);
+// jpeg_forward_dev without the launch: the job's buffers and the block stage's parameters
+int jpeg_forward_plan(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag, const int* rows,
+                      Fdct8Params* P);
 // Enqueue entropy coding on the device + async copy of the scan to pinned memory.
 int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job);
 // second phase, once the stream was synchronised and the sizes are on the host
 int jpeg_entropy_fetch(Workspace& ws, JpegEncodeJob* job);
+// Entropy coding of many JPEGs with one launch (k_huff_encode_batch): each job gets the segment jpeg_entropy_dev gives
+// it, one chunk size for all of them.  Enqueued on ws.stream() with one copy of every job's control words to pinned
+// memory (job->h_scan_bytes).  jpeg_entropy_batch_fetch, once the stream was synchronised: one launch gathers the
+// segments into one buffer and one copy brings it to pinned memory (job->h_scan; null for a scan that overflowed).
+int jpeg_entropy_batch_dev(Workspace& ws, JpegEncodeJob* const* jobs, int n);
+int jpeg_entropy_batch_fetch(Workspace& ws, JpegEncodeJob* const* jobs, int n);
+// since process start: [0] k_huff_encode_batch launches, [1] scans they coded
+void jpeg_encode_batch_stats(unsigned long long out[2]);
 // k_huff_encode plans since process start: [0] resident CTAs per wave, [1..8] launches by blocks per thread,
 // [9] launches whose grid exceeded one wave
 void jpeg_encode_stats(unsigned long long out[10]);

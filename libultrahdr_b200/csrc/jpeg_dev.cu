@@ -8,11 +8,20 @@
 namespace uhdr_b200 {
 
 int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag, const int* rows) {
+  Fdct8Params P;
+  const int rc = jpeg_forward_plan(ws, img, quality, job, zigzag, rows, &P);
+  if (rc) return rc;
+  TIMED(ws, "fdct_quant", launch_fdct8(P, ws.stream()));
+  return E_OK;
+}
+
+int jpeg_forward_plan(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag, const int* rows,
+                      Fdct8Params* out) {
   int rc = jpeg_frame_init(&job->frame, img.v.fmt, img.v.w, img.v.h, quality);
   if (rc) return rc;
   const JpegFrame& f = job->frame;
   job->zigzag = zigzag;
-  Fdct8Params P;
+  Fdct8Params& P = *out;
   memset(&P, 0, sizeof P);
   P.zigzag = zigzag ? 1 : 0;
   memcpy(P.q[0], f.qt[0], sizeof P.q[0]);
@@ -72,7 +81,6 @@ int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncode
       pl.hsel[0] = c == 0 ? 0 : 1;
     }
   }
-  TIMED(ws, "fdct_quant", launch_fdct8(P, ws.stream()));
   return E_OK;
 }
 

@@ -238,6 +238,10 @@ cudaError_t launch_yuv420_fast(const YuvConvParams& p, cudaStream_t s);
 cudaError_t launch_rgb_to_ycc(const RgbToYccParams& p, cudaStream_t s);
 cudaError_t launch_resize_map(const ResizeMapParams& p, cudaStream_t s);
 cudaError_t launch_fdct8(const Fdct8Params& p, cudaStream_t s);
+// k_fdct8_code_batch: planes / item_end (cumulative ceil(blocks / 32) warp items, `total_items` its last entry) in device
+// memory, no RGB888 plane; plane.tq[0] selects q[0..3]
+cudaError_t launch_fdct8_code_batch(const Fdct8Plane* planes, const unsigned* item_end, unsigned nplanes, unsigned total_items,
+                                    const uint16_t q[4][64], cudaStream_t s);
 cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s);
 cudaError_t launch_idct_scaled(const IdctScaledParams& p, int size, cudaStream_t s);
 // planes / cta_end: n entries in device memory, cta_end the inclusive prefix of the planes' ceil(blocks / 128) CTAs,

@@ -21,9 +21,8 @@ struct Ycc420Params {
   int dy_stride, dc_stride, lw, lh, cw, ch;
 };
 
-__global__ void k_ycc444_to_420(const Ycc420Params p) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y * blockDim.y + threadIdx.y;
-  if (j >= p.cw || i >= p.ch) return;
+// chroma sample (j, i), j < cw, i < ch: that sample of both chroma planes and the 2x2 luma samples above it
+__device__ __forceinline__ void ycc444_to_420_at(const Ycc420Params& p, const int j, const int i) {
 #pragma unroll
   for (int dy = 0; dy < 2; dy++) {
     const int yy = 2 * i + dy;
@@ -41,6 +40,46 @@ __global__ void k_ycc444_to_420(const Ycc420Params p) {
   const size_t o = (size_t)i * p.dc_stride + j;
   p.dcb[o] = (uint8_t)((__ldg(p.cb + r0 + c0) + __ldg(p.cb + r0 + c1) + __ldg(p.cb + r1 + c0) + __ldg(p.cb + r1 + c1) + bias) >> 2);
   p.dcr[o] = (uint8_t)((__ldg(p.cr + r0 + c0) + __ldg(p.cr + r0 + c1) + __ldg(p.cr + r1 + c0) + __ldg(p.cr + r1 + c1) + bias) >> 2);
+}
+
+__global__ void k_ycc444_to_420(const Ycc420Params p) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y * blockDim.y + threadIdx.y;
+  if (j >= p.cw || i >= p.ch) return;
+  ycc444_to_420_at(p, j, i);
+}
+
+// One image plane (or, with `ycc420`, one 4:2:0 input image) of k_stage_batch: the bytes the block stage reads.
+//  * plane: stage_tight + helper_padding of a decoded plane pw x ph (src, src_stride) into dst (dst_stride): columns
+//    [pw, aw) hold `fill` (0 luma, 128 chroma), and when pw < aw the rows [ph, rows) are the helper's scratch rows --
+//    the row one iMCU (imcu rows) above, or inside the first iMCU 0 up to pw and `fill` after it.  width = aw.
+//  * ycc420: libjpeg's 4:2:0 input stage of a 4:4:4 image, k_ycc444_to_420's bytes; width = cw, one thread per chroma
+//    sample.
+struct StageJob {
+  Ycc420Params p;
+  const uint8_t* src;
+  uint8_t* dst;
+  int src_stride, dst_stride, pw, ph, aw, rows, fill, imcu;
+  int ycc420, width;
+};
+
+// every plane of a group in one launch: 256 work items (bytes; chroma samples of a ycc420 job) per CTA, the job found
+// by a binary search over the jobs' cumulative CTA counts
+__global__ void __launch_bounds__(256) k_stage_batch(const StageJob* __restrict__ jobs, const unsigned* __restrict__ cta_end,
+                                                     unsigned njobs) {
+  const unsigned ji = batch_find(cta_end, njobs, blockIdx.x);
+  const StageJob& J = jobs[ji];
+  const unsigned idx = (blockIdx.x - (ji ? cta_end[ji - 1] : 0u)) * 256u + threadIdx.x;
+  const int y = (int)(idx / (unsigned)J.width), x = (int)(idx - (unsigned)y * J.width);
+  if (J.ycc420) {
+    if (y < J.p.ch) ycc444_to_420_at(J.p, x, y);
+    return;
+  }
+  if (y >= J.rows) return;
+  int sy = y;
+  while (sy >= J.ph && sy >= J.imcu) sy -= J.imcu;   // helper_padding copies the row one iMCU up
+  uint8_t v = (uint8_t)J.fill;
+  if (x < J.pw) v = sy < J.ph ? __ldg(J.src + (size_t)sy * J.src_stride + x) : (uint8_t)0;
+  J.dst[(size_t)y * J.dst_stride + x] = v;
 }
 
 cudaError_t launch_ycc444_to_420(const Ycc420Params& p, cudaStream_t s) {
@@ -125,7 +164,7 @@ int JpegRCodec::transcode(const uint8_t* data, size_t size, const DecodedInfo& p
   JpegEncodeJob base_jpeg, gm_jpeg;
   if (!rc) {
     if (cfg.base_420 && sdr.v.fmt == F_YUV422)
-      rc = fail(E_UNSUPPORTED, "a 4:2:0 base image is written from 4:4:4 or 4:2:0 input, the base image is 4:2:2");
+      rc = fail_base_422();
     else if (cfg.base_420 && sdr.v.fmt == F_YUV444)
       rc = ycc444_to_420_dev(ws_, sdr, &base_in, base_rows);
     else
@@ -146,6 +185,18 @@ int JpegRCodec::transcode(const uint8_t* data, size_t size, const DecodedInfo& p
     return rc;
   }
   tr.mark("scans on the host");
+  rc = transcode_finish(data, probed, ph, gh, base_jpeg, gm_jpeg, cfg, out, cap, out_size);
+  if (!rc) tr.mark("file assembled");
+  return rc;
+}
+
+int JpegRCodec::fail_base_422() {
+  return fail(E_UNSUPPORTED, "a 4:2:0 base image is written from 4:4:4 or 4:2:0 input, the base image is 4:2:2");
+}
+
+int JpegRCodec::transcode_finish(const uint8_t* data, const DecodedInfo& probed, const JpegHeader& ph, const JpegHeader& gh,
+                                 const JpegEncodeJob& base_jpeg, const JpegEncodeJob& gm_jpeg,
+                                 const uhdr_b200_transcode_config_t& cfg, uint8_t* out, size_t cap, size_t* out_size) {
   const uint8_t* pd = data + probed.base_off;
   const uint8_t* gd = data + probed.gainmap_off;
   const ByteView base_icc = find_marker(pd, ph, 0xE2, "ICC_PROFILE", 12), gm_icc = find_marker(gd, gh, 0xE2, "ICC_PROFILE", 12);
@@ -157,17 +208,19 @@ int JpegRCodec::transcode(const uint8_t* data, size_t size, const DecodedInfo& p
   const uint8_t* add_icc = nullptr;
   size_t add_icc_n = 0;
   if (base_icc.empty()) {
-    if (sdr.cg <= UHDR_CG_UNSPECIFIED || sdr.cg > UHDR_CG_BT_2100) return fail(E_INVALID_PARAM, "Unrecognized 420 color gamut %d", sdr.cg);
-    add_icc = icc_profile(UHDR_CT_SRGB, sdr.cg, &add_icc_n);
+    const int cg = icc_read_gamut(base_icc.data, base_icc.size);   // the primary image's gamut as the decode gives it
+    if (cg <= UHDR_CG_UNSPECIFIED || cg > UHDR_CG_BT_2100) return fail(E_INVALID_PARAM, "Unrecognized 420 color gamut %d", cg);
+    add_icc = icc_profile(UHDR_CT_SRGB, cg, &add_icc_n);
   }
-  const char* base_com = base_in.v.fmt == F_Y400 ? jpeg_gainmap_comment() : nullptr;
-  const char* gm_com = map_in.v.fmt == F_Y400 ? jpeg_gainmap_comment() : nullptr;
+  const char* base_com = base_jpeg.frame.ncomp == 1 ? jpeg_gainmap_comment() : nullptr;
+  const char* gm_com = gm_jpeg.frame.ncomp == 1 ? jpeg_gainmap_comment() : nullptr;
   JpegPieces pb, pg;
   const size_t base_cap = jpeg_head_capacity(base_icc.size, base_com), gm_cap = jpeg_head_capacity(gm_icc.size, gm_com);
   uint8_t* base_head = (uint8_t*)ws_.halloc(base_cap);
   uint8_t* gm_head = (uint8_t*)ws_.halloc(gm_cap);
   if (!base_head || !gm_head) return E_MEM;
-  rc = jpeg_stream_pieces(base_jpeg, base_icc.data, base_icc.size, base_com, base_head, base_cap, &pb.head_len, &pb.scan, &pb.scan_len);
+  int rc = jpeg_stream_pieces(base_jpeg, base_icc.data, base_icc.size, base_com, base_head, base_cap, &pb.head_len, &pb.scan,
+                              &pb.scan_len);
   if (rc) return rc;
   rc = jpeg_stream_pieces(gm_jpeg, gm_icc.data, gm_icc.size, gm_com, gm_head, gm_cap, &pg.head_len, &pg.scan, &pg.scan_len);
   if (rc) return rc;
@@ -186,7 +239,287 @@ int JpegRCodec::transcode(const uint8_t* data, size_t size, const DecodedInfo& p
   *out_size = n;
   if (n > cap) return fail(E_MEM, "output buffer of %zu bytes is too small for the encoded stream of %zu bytes", cap, n);
   memcpy(out, file, n);
-  tr.mark("file assembled");
+  return E_OK;
+}
+
+namespace {
+
+void item_fail(TranscodeBatchItem& it, int rc, const char* msg) {
+  it.rc = rc;
+  snprintf(it.err, sizeof it.err, "%s", msg);
+}
+
+// a workspace plane of aw x rows bytes for the block stage
+int stage_plane(Workspace& ws, int aw, int rows, uint8_t** out) {
+  *out = (uint8_t*)ws.dalloc((size_t)aw * rows);
+  return *out ? E_OK : E_MEM;
+}
+
+// stage_tight's (and helper_padding's) bytes of `src` as k_stage_batch jobs into a new image *out; rows[c] as there
+int plan_stage_tight(Workspace& ws, const DevImage& src, StageJob* jobs, int* nj, DevImage* out, int rows[3]) {
+  memset(out, 0, sizeof *out);
+  out->v = src.v;
+  for (int i = 0; i < fmt_planes(src.v.fmt); i++) {
+    int pw, ph, esz;
+    fmt_plane_geom(src.v.fmt, src.v.w, src.v.h, i, &pw, &ph, &esz);
+    const int aw = (pw + 7) / 8 * 8;
+    StageJob& J = jobs[(*nj)++];
+    memset(&J, 0, sizeof J);
+    J.src = (const uint8_t*)src.v.p[i];
+    J.src_stride = src.v.stride[i];
+    J.pw = pw;
+    J.ph = ph;
+    J.aw = J.width = aw;
+    J.rows = rows[i] = pw == aw ? ph : (ph + 7) / 8 * 8;
+    J.fill = i == 0 ? 0 : 128;
+    J.imcu = (src.v.fmt == F_YUV420 && i == 0) ? 16 : 8;
+    J.dst_stride = aw;
+    int rc = stage_plane(ws, aw, J.rows, &J.dst);
+    if (rc) return rc;
+    out->v.p[i] = J.dst;
+    out->v.stride[i] = aw;
+  }
+  return E_OK;
+}
+
+// ycc444_to_420_dev's bytes as one k_stage_batch job
+int plan_ycc444_to_420(Workspace& ws, const DevImage& src, StageJob* jobs, int* nj, DevImage* out, int rows[3]) {
+  JpegFrame f;
+  int rc = jpeg_frame_init(&f, F_YUV420, src.v.w, src.v.h, 75);
+  if (rc) return rc;
+  StageJob& J = jobs[(*nj)++];
+  memset(&J, 0, sizeof J);
+  Ycc420Params& p = J.p;
+  p.y = (const uint8_t*)src.v.p[0];
+  p.cb = (const uint8_t*)src.v.p[1];
+  p.cr = (const uint8_t*)src.v.p[2];
+  p.src_stride = src.v.stride[0];
+  p.w = src.v.w;
+  p.h = src.v.h;
+  p.lw = f.comp[0].wblocks * 8;
+  p.lh = f.comp[0].hblocks * 8;
+  p.cw = f.comp[1].wblocks * 8;
+  p.ch = f.comp[1].hblocks * 8;
+  p.dy_stride = p.lw;
+  p.dc_stride = p.cw;
+  uint8_t* planes[3];
+  if ((rc = stage_plane(ws, p.lw, p.lh, &planes[0])) || (rc = stage_plane(ws, p.cw, p.ch, &planes[1])) ||
+      (rc = stage_plane(ws, p.cw, p.ch, &planes[2])))
+    return rc;
+  p.dy = planes[0];
+  p.dcb = planes[1];
+  p.dcr = planes[2];
+  J.ycc420 = 1;
+  J.width = p.cw;
+  rows[0] = p.lh;
+  rows[1] = rows[2] = p.ch;
+  memset(out, 0, sizeof *out);
+  out->v.fmt = F_YUV420;
+  out->v.w = src.v.w;
+  out->v.h = src.v.h;
+  out->v.full_range = 1;
+  for (int c = 0; c < 3; c++) {
+    out->v.p[c] = planes[c];
+    out->v.stride[c] = c ? p.cw : p.lw;
+  }
+  return E_OK;
+}
+
+// one H2D copy of a host plan array into workspace device memory
+template <class T>
+int upload_plan(Workspace& ws, const T* h, size_t n, T** d) {
+  *d = (T*)ws.dalloc(sizeof(T) * n);
+  if (!*d) return E_MEM;
+  CUDA_TRY(cudaMemcpyAsync(*d, h, sizeof(T) * n, cudaMemcpyHostToDevice, ws.stream()));
+  return E_OK;
+}
+
+}  // namespace
+
+size_t JpegRCodec::batch_decode_bytes(int w, int h, int gw, int gh, int k, size_t size) {
+  // coefficients (128 B per 8x8 block, at most 3 components at full size) and their DC terms, planes, coded bits
+  const size_t px = (size_t)w * k * h * k + (size_t)gw * k * gh * k;
+  return px * 7 + (size_t)(w * h + gw * gh) * 16 + 2 * size;
+}
+
+int JpegRCodec::transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg, size_t group_bytes) {
+  int rc = settle();
+  if (rc) return rc;
+  map_pending_ = false;
+  const int k = cfg.k;
+  auto cost = [&](int i, size_t* coded) {
+    const DecodedInfo& in = items[i].info;
+    *coded = items[i].size;
+    const int w = (in.width + k - 1) / k, h = (in.height + k - 1) / k, gw = (in.gm_width + k - 1) / k,
+              gh = (in.gm_height + k - 1) / k;
+    size_t enc = 0;
+    for (int j = 0; j < 2; j++) {   // per JPEG: staged planes, 256 B of code-word entries and 16 B of meta per block, the scan
+      const size_t pw = j ? gw : w, ph = j ? gh : h, blocks = 3 * ((pw + 15) / 8) * ((ph + 15) / 8);
+      enc += 3 * (pw + 8) * (ph + 16) + blocks * (256 + 16) + pw * ph * 6 + 8192;
+    }
+    return batch_decode_bytes(w, h, gw, gh, k, items[i].size) + enc;
+  };
+  rc = for_each_group(n, group_bytes, cost, [&](int g0, int g1) { return transcode_batch_group(items + g0, g1 - g0, cfg); });
+  if (rc) mark_in_flight();   // as transcode(): kernels of the group may still run
+  return rc;
+}
+
+int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg) {
+  const int k = cfg.k;
+  int rc = E_OK;
+  // 1. per item, the header stages of both JPEGs (decode_pair's order: primary, then map), raw planes for both
+  if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
+  if ((int)batch_idct_.size() < 2 * n) batch_idct_.resize(2 * n);
+  if ((int)batch_enc_.size() < 2 * n) batch_enc_.resize(2 * n);
+  JpegBatchScan* scans = batch_scans_.data();
+  int ns = 0;
+  for (int i = 0; i < n; i++) {
+    TranscodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    const DecodedInfo& in = it.info;
+    it.map_rc = E_OK;
+    rc = decode_jpeg_begin(ws_, it.data + in.base_off, in.base_len, 0, k, &it.sdr, &it.ph, &it.pj);
+    if (rc == E_MEM) return rc;
+    if (rc) {
+      item_fail(it, rc, last_error());
+      continue;
+    }
+    scans[ns++] = JpegBatchScan{it.data + in.base_off, in.base_len, &it.ph, {}, 0, {0}};
+    it.map_rc = decode_jpeg_begin(ws_, it.data + in.gainmap_off, in.gainmap_len, 0, k, &it.map, &it.gh, &it.gj);
+    if (it.map_rc == E_MEM) return E_MEM;
+    if (it.map_rc) snprintf(it.map_err, sizeof it.map_err, "%s", last_error());
+    else scans[ns++] = JpegBatchScan{it.data + in.gainmap_off, in.gainmap_len, &it.gh, {}, 0, {0}};
+  }
+  // 2. entropy decoding of every scan
+  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
+  // 3. in the order transcode() meets them: the primary's result and its tail stage, the map header's error, the map's
+  // result and tail stage, the 4:2:2 check of base_420; then one inverse DCT for everything that is left
+  JpegIdctJob* jobs = batch_idct_.data();
+  int nj = 0, si = 0;
+  auto add_job = [&](const JpegHeader& h, const JpegDecodeJob& j, const JpegBatchScan& sc) {
+    JpegIdctJob& o = jobs[nj++];
+    o.h = &h;
+    o.g = j.k != 1 ? &j.g : nullptr;
+    for (int c = 0; c < 3; c++) {
+      o.d_coefs[c] = sc.d_coefs[c];
+      o.planes[c] = j.planes[c];
+      o.strides[c] = j.strides[c];
+    }
+  };
+  for (int i = 0; i < n; i++) {
+    TranscodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    const JpegBatchScan& ps = scans[si++];
+    const JpegBatchScan* gs = !it.map_rc ? &scans[si++] : nullptr;
+    int r = ps.rc;
+    if (r) {
+      item_fail(it, r, ps.err);
+      continue;
+    }
+    if ((r = decode_jpeg_end(ws_, &it.ph, it.pj, &it.sdr, nullptr))) {
+      if (r == E_MEM) return r;
+      item_fail(it, r, last_error());
+      continue;
+    }
+    if (it.map_rc) {
+      item_fail(it, it.map_rc, it.map_err);
+      continue;
+    }
+    if (gs->rc) {
+      item_fail(it, gs->rc, gs->err);
+      continue;
+    }
+    if ((r = decode_jpeg_end(ws_, &it.gh, it.gj, &it.map, nullptr))) {
+      if (r == E_MEM) return r;
+      item_fail(it, r, last_error());
+      continue;
+    }
+    if (cfg.base_420 && it.sdr.v.fmt == F_YUV422) {
+      item_fail(it, fail_base_422(), last_error());
+      continue;
+    }
+    add_job(it.ph, it.pj, ps);
+    add_job(it.gh, it.gj, *gs);
+  }
+  if (nj && (rc = jpeg_idct_batch_dev(ws_, jobs, nj))) return rc;
+  // 4. the staging jobs and the block stage's planes of both JPEGs of every item: base quantisers 0 / 1, map's 2 / 3
+  StageJob* h_stage = (StageJob*)ws_.halloc(sizeof(StageJob) * 6 * n);
+  unsigned* h_stage_end = (unsigned*)ws_.halloc(sizeof(unsigned) * 6 * n);
+  Fdct8Plane* h_pl = (Fdct8Plane*)ws_.halloc(sizeof(Fdct8Plane) * 6 * n);
+  unsigned* h_pl_end = (unsigned*)ws_.halloc(sizeof(unsigned) * 6 * n);
+  if (!h_stage || !h_stage_end || !h_pl || !h_pl_end) return E_MEM;
+  uint16_t q[4][64];
+  memset(q, 0, sizeof q);
+  int nst = 0, npl = 0, nenc = 0;
+  unsigned items_total = 0;
+  JpegEncodeJob** enc = batch_enc_.data();
+  for (int i = 0; i < n; i++) {
+    TranscodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    DevImage base_in, map_in;
+    int base_rows[3], map_rows[3];
+    const int nst0 = nst;
+    int r = cfg.base_420 && it.sdr.v.fmt == F_YUV444 ? plan_ycc444_to_420(ws_, it.sdr, h_stage, &nst, &base_in, base_rows)
+                                                     : plan_stage_tight(ws_, it.sdr, h_stage, &nst, &base_in, base_rows);
+    if (!r) r = plan_stage_tight(ws_, it.map, h_stage, &nst, &map_in, map_rows);
+    Fdct8Params P[2];
+    if (!r) r = jpeg_forward_plan(ws_, base_in, cfg.base_quality, &it.base_jpeg, /*zigzag=*/true, base_rows, &P[0]);
+    if (!r) r = jpeg_forward_plan(ws_, map_in, cfg.gainmap_quality, &it.gm_jpeg, /*zigzag=*/true, map_rows, &P[1]);
+    if (r == E_MEM) return r;
+    if (r) {
+      nst = nst0;
+      item_fail(it, r, last_error());
+      continue;
+    }
+    for (int j = 0; j < 2; j++) {
+      memcpy(q[2 * j], P[j].q, sizeof P[j].q);
+      for (int c = 0; c < P[j].nplanes; c++) {
+        Fdct8Plane& pl = h_pl[npl];
+        pl = P[j].plane[c];
+        pl.tq[0] += 2 * j;
+        items_total += (unsigned)(pl.wblocks * pl.hblocks + 31) / 32;
+        h_pl_end[npl++] = items_total;
+      }
+    }
+    enc[nenc++] = &it.base_jpeg;
+    enc[nenc++] = &it.gm_jpeg;
+  }
+  if (!nenc) return E_OK;
+  unsigned ctas = 0;
+  for (int j = 0; j < nst; j++) {
+    const StageJob& J = h_stage[j];
+    ctas += (unsigned)(((size_t)J.width * (J.ycc420 ? J.p.ch : J.rows) + 255) / 256);
+    h_stage_end[j] = ctas;
+  }
+  // 5. one staging launch, one block-stage launch, one entropy-coding launch for the whole group
+  StageJob* d_stage;
+  unsigned *d_stage_end, *d_pl_end;
+  Fdct8Plane* d_pl;
+  if ((rc = upload_plan(ws_, h_stage, nst, &d_stage)) || (rc = upload_plan(ws_, h_stage_end, nst, &d_stage_end)) ||
+      (rc = upload_plan(ws_, h_pl, npl, &d_pl)) || (rc = upload_plan(ws_, h_pl_end, npl, &d_pl_end)))
+    return rc;
+  count_launches(1);
+  ws_.t_begin("stage_batch");
+  k_stage_batch<<<ctas, 256, 0, ws_.stream()>>>(d_stage, d_stage_end, (unsigned)nst);
+  ws_.t_end();
+  CUDA_TRY(cudaGetLastError());
+  TIMED(ws_, "fdct_code_batch", launch_fdct8_code_batch(d_pl, d_pl_end, (unsigned)npl, items_total, q, ws_.stream()));
+  if ((rc = jpeg_entropy_batch_dev(ws_, enc, nenc))) return rc;
+  // 6. two host waits: every scan's size, then every scan's bytes
+  if ((rc = ws_.sync())) return rc;
+  if ((rc = jpeg_entropy_batch_fetch(ws_, enc, nenc))) return rc;
+  if ((rc = ws_.sync())) return rc;
+  // 7. per item, the file
+  for (int i = 0; i < n; i++) {
+    TranscodeBatchItem& it = items[i];
+    if (it.rc) continue;
+    int r = E_OK;
+    for (const JpegEncodeJob* j : {&it.base_jpeg, &it.gm_jpeg})
+      if (!r && j->h_scan_bytes[4])
+        r = fail(E_MEM, "entropy-coded segment exceeds the %zu byte device buffer", j->scan_capacity);
+    if (!r) r = transcode_finish(it.data, it.info, it.ph, it.gh, it.base_jpeg, it.gm_jpeg, cfg, it.out, it.cap, &it.out_size);
+    if (r) item_fail(it, r, last_error());
+  }
   return E_OK;
 }
 

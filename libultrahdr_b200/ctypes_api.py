@@ -166,3 +166,25 @@ def declare_transcode(lib):
     lib.uhdr_b200_transcode.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(TranscodeConfig), C.c_void_p, C.c_size_t,
                                         C.POINTER(C.c_size_t)]
     return lib
+
+
+class TranscodeItem(C.Structure):
+    """uhdr_b200_transcode_item_t: one file of uhdr_b200_transcode_batch"""
+    _fields_ = [("data", C.c_void_p), ("size", C.c_size_t), ("out", C.c_void_p), ("cap", C.c_size_t),
+                ("out_size", C.c_size_t), ("status", C.c_int)]
+
+
+def declare_transcode_batch(lib):
+    """argument types of uhdr_b200_transcode_batch and uhdr_b200_jpeg_encode_batch_stats (include/uhdr_b200.h) on a
+    loaded libuhdr_b200"""
+    lib.uhdr_b200_transcode_batch.argtypes = [C.POINTER(TranscodeItem), C.c_int, C.POINTER(TranscodeConfig)]
+    lib.uhdr_b200_jpeg_encode_batch_stats.argtypes = [C.POINTER(C.c_ulonglong)]
+    lib.uhdr_b200_jpeg_encode_batch_stats.restype = None
+    return lib
+
+
+def jpeg_encode_batch_stats(lib):
+    """-> (k_huff_encode_batch launches, scans they coded) since process start"""
+    st = (C.c_ulonglong * 2)()
+    lib.uhdr_b200_jpeg_encode_batch_stats(st)
+    return st[0], st[1]
