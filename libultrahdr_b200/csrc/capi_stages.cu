@@ -375,6 +375,39 @@ int check_dev_memory(const uhdr_raw_image_t& img, const char* what) {
   return E_OK;
 }
 }  // namespace uhdr_b200
+
+namespace {
+// The batched entry points' items: grow-only per thread and item type, so a batch of the same or a smaller size
+// takes no heap
+template <class Item>
+Item* batch_items(int n) {
+  static thread_local std::vector<Item> its;
+  if ((int)its.size() < n) its.resize(n);
+  return its.data();
+}
+
+// The batched entry points' tail: run(group bytes) unless `rc` (dev_codec's code) already ends the call, that call-level
+// error given to every item without one of its own, each item's status, and the first failing item's code and message
+template <class In, class Item, class Run>
+int run_batch(In* items, Item* its, int n, int rc, Run run) {
+  if (!rc) {
+    size_t group = size_t(4) << 30;
+    if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
+    rc = run(group);
+  }
+  std::string call_err = rc ? last_error() : "";
+  int first = -1;
+  for (int i = 0; i < n; i++) {
+    Item& b = its[i];
+    if (rc && !b.rc) batch_fail(b, rc, call_err.c_str());
+    items[i].status = b.rc;
+    if (b.rc && first < 0) first = i;
+  }
+  if (first < 0) return E_OK;
+  return fail(its[first].rc, "item %d: %s", first, its[first].err);
+}
+}  // namespace
+
 extern "C" {
 namespace {
 bool valid_scale(int k) { return k == 1 || k == 2 || k == 4 || k == 8; }
@@ -464,8 +497,7 @@ UHDR_API int uhdr_b200_decode_batch_dev(uhdr_b200_decode_item_t* items, int n, i
   if (!items) return fail(E_INVALID_PARAM, "received nullptr for the items");
   if (n < 1) return fail(E_INVALID_PARAM, "received %d items, expects at least 1", n);
   if (!valid_scale(k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", k);
-  static thread_local std::vector<DecodeBatchItem> its;  // grow-only: a batch of the same or a smaller size takes no heap
-  if ((int)its.size() < n) its.resize(n);
+  DecodeBatchItem* its = batch_items<DecodeBatchItem>(n);
   for (int i = 0; i < n; i++) {
     const uhdr_b200_decode_item_t& in = items[i];
     DecodeBatchItem& b = its[i];
@@ -478,29 +510,13 @@ UHDR_API int uhdr_b200_decode_batch_dev(uhdr_b200_decode_item_t* items, int n, i
     if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
   }
   JpegRCodec* c = nullptr;
-  int rc = dev_codec(&c);
-  for (int i = 0; i < n && !rc; i++) {
-    DecodeBatchItem& b = its[i];
-    if (!b.rc && (b.rc = check_decode_memory(b.dest, b.gainmap, b.info))) snprintf(b.err, sizeof b.err, "%s", last_error());
-  }
-  if (!rc) {
-    size_t group = size_t(4) << 30;
-    if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
-    rc = c->decode_batch(its.data(), n, k, out_ct, max_display_boost, (cudaStream_t)stream, group);
-  }
-  std::string call_err = rc ? last_error() : "";
-  int first = -1;
-  for (int i = 0; i < n; i++) {
-    DecodeBatchItem& b = its[i];
-    if (rc && !b.rc) {  // an error of the whole call: every item without its own
-      b.rc = rc;
-      snprintf(b.err, sizeof b.err, "%s", call_err.c_str());
+  return run_batch(items, its, n, dev_codec(&c), [&](size_t group) {
+    for (int i = 0; i < n; i++) {
+      DecodeBatchItem& b = its[i];
+      if (!b.rc && (b.rc = check_decode_memory(b.dest, b.gainmap, b.info))) snprintf(b.err, sizeof b.err, "%s", last_error());
     }
-    items[i].status = b.rc;
-    if (b.rc && first < 0) first = i;
-  }
-  if (first < 0) return E_OK;
-  return fail(its[first].rc, "item %d: %s", first, its[first].err);
+    return c->decode_batch(its, n, k, out_ct, max_display_boost, (cudaStream_t)stream, group);
+  });
 }
 
 UHDR_API int uhdr_b200_scaled_dims(const void* data, size_t size, int k, unsigned* w, unsigned* h, unsigned* gm_w,
@@ -593,8 +609,7 @@ UHDR_API int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n,
   if (!valid_scale(cfg->k)) return fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", cfg->k);
   if (cfg->base_quality < 0 || cfg->base_quality > 100 || cfg->gainmap_quality < 0 || cfg->gainmap_quality > 100)
     return fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", cfg->base_quality, cfg->gainmap_quality);
-  static thread_local std::vector<TranscodeBatchItem> its;  // grow-only: a batch of the same or a smaller size takes no heap
-  if ((int)its.size() < n) its.resize(n);
+  TranscodeBatchItem* its = batch_items<TranscodeBatchItem>(n);
   for (int i = 0; i < n; i++) {
     const uhdr_b200_transcode_item_t& in = items[i];
     TranscodeBatchItem& b = its[i];
@@ -610,27 +625,10 @@ UHDR_API int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n,
     if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
   }
   JpegRCodec* c = nullptr;
-  int rc = dev_codec(&c);
-  if (!rc) {
-    size_t group = size_t(4) << 30;
-    if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
-    rc = c->transcode_batch(its.data(), n, *cfg, group);
-  }
-  std::string call_err = rc ? last_error() : "";
-  int first = -1;
-  for (int i = 0; i < n; i++) {
-    TranscodeBatchItem& b = its[i];
-    if (rc && !b.rc) {  // an error of the whole call: every item without its own
-      b.rc = rc;
-      snprintf(b.err, sizeof b.err, "%s", call_err.c_str());
-    }
-    items[i].status = b.rc;
-    // out_size: bytes written, or with UHDR_CODEC_MEM_ERROR the size needed (0 when the file was not assembled)
-    items[i].out_size = !b.rc || b.rc == E_MEM ? b.out_size : 0;
-    if (b.rc && first < 0) first = i;
-  }
-  if (first < 0) return E_OK;
-  return fail(its[first].rc, "item %d: %s", first, its[first].err);
+  const int rc = run_batch(items, its, n, dev_codec(&c), [&](size_t group) { return c->transcode_batch(its, n, *cfg, group); });
+  // out_size: bytes written, or with UHDR_CODEC_MEM_ERROR the size needed (0 when the file was not assembled)
+  for (int i = 0; i < n; i++) items[i].out_size = !its[i].rc || its[i].rc == E_MEM ? its[i].out_size : 0;
+  return rc;
 }
 
 UHDR_API int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img, int quality, const void* icc, size_t icc_size, void* out,

@@ -845,10 +845,93 @@ int JpegRCodec::enqueue_dev_writes(const DevImage& sdr, const DevImage& map, con
   return E_OK;
 }
 
-static void batch_item_fail(DecodeBatchItem& it, int rc, const char* msg) {
-  it.rc = rc;
-  snprintf(it.err, sizeof it.err, "%s", msg);
+template <class Item>
+int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool defer_rgba, int map_mode) {
+  int rc = E_OK;
+  // 1. per file, the header stages of both JPEGs (decode_pair's order: primary, then map)
+  if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
+  if ((int)batch_idct_.size() < 2 * n) batch_idct_.resize(2 * n);
+  JpegBatchScan* scans = batch_scans_.data();
+  int ns = 0;
+  for (int i = 0; i < n; i++) {
+    BatchFile& f = items[i];
+    if (f.rc) continue;
+    const DecodedInfo& in = f.info;
+    f.map_rc = E_OK;
+    rc = decode_jpeg_begin(ws_, f.data + in.base_off, in.base_len, sdr_mode, k, &f.sdr, &f.ph, &f.pj);
+    if (rc == E_MEM) return rc;
+    if (rc) {
+      batch_fail(f, rc, last_error());
+      continue;
+    }
+    scans[ns++] = JpegBatchScan{f.data + in.base_off, in.base_len, &f.ph, {}, 0, {0}};
+    if (!f.want_map) continue;
+    f.map_rc = decode_jpeg_begin(ws_, f.data + in.gainmap_off, in.gainmap_len, map_mode, k, &f.map, &f.gh, &f.gj);
+    if (f.map_rc == E_MEM) return E_MEM;
+    if (f.map_rc) snprintf(f.map_err, sizeof f.map_err, "%s", last_error());
+    else scans[ns++] = JpegBatchScan{f.data + in.gainmap_off, in.gainmap_len, &f.gh, {}, 0, {0}};
+  }
+  // 2. entropy decoding of every scan
+  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
+  // 3. in the order the single call meets them: the primary's result and its tail stage (which launches nothing for
+  // these modes), the map header's error, the map's result; then one inverse DCT for everything that is left
+  JpegIdctJob* jobs = batch_idct_.data();
+  int nj = 0, si = 0;
+  auto add_job = [&](const JpegHeader& h, const JpegDecodeJob& j, const JpegBatchScan& sc) {
+    JpegIdctJob& o = jobs[nj++];
+    o.h = &h;
+    o.g = j.k != 1 ? &j.g : nullptr;
+    for (int c = 0; c < 3; c++) {
+      o.d_coefs[c] = sc.d_coefs[c];
+      o.planes[c] = j.planes[c];
+      o.strides[c] = j.strides[c];
+    }
+  };
+  for (int i = 0; i < n; i++) {
+    BatchFile& f = items[i];
+    if (f.rc) continue;
+    const JpegBatchScan& ps = scans[si++];
+    const JpegBatchScan* gs = f.want_map && !f.map_rc ? &scans[si++] : nullptr;
+    if (ps.rc) {
+      batch_fail(f, ps.rc, ps.err);
+      continue;
+    }
+    if (int r = decode_jpeg_end(ws_, &f.ph, f.pj, &f.sdr, defer_rgba ? &f.to_rgba : nullptr)) {
+      if (r == E_MEM) return r;
+      batch_fail(f, r, last_error());
+      continue;
+    }
+    if (f.map_rc) {
+      batch_fail(f, f.map_rc, f.map_err);
+      continue;
+    }
+    if (gs && gs->rc) {
+      batch_fail(f, gs->rc, gs->err);
+      continue;
+    }
+    add_job(f.ph, f.pj, ps);
+    if (gs) add_job(f.gh, f.gj, *gs);
+  }
+  if (nj && (rc = jpeg_idct_batch_dev(ws_, jobs, nj))) return rc;
+  // 4. per file, the map's tail stage -- after the inverse DCT: a 3-channel map in mode 2 launches its colour conversion
+  // there -- and the gamuts of both ICC profiles
+  for (int i = 0; i < n; i++) {
+    BatchFile& f = items[i];
+    if (f.rc) continue;
+    ByteView blob = find_marker(f.data + f.info.base_off, f.ph, 0xE2, "ICC_PROFILE", 12);
+    f.sdr.cg = icc_read_gamut(blob.data, blob.size);
+    if (!f.want_map) continue;
+    if (int r = decode_jpeg_end(ws_, &f.gh, f.gj, &f.map, nullptr)) {
+      if (r == E_MEM) return r;
+      batch_fail(f, r, last_error());
+      continue;
+    }
+    blob = find_marker(f.data + f.info.gainmap_off, f.gh, 0xE2, "ICC_PROFILE", 12);
+    f.map.cg = icc_read_gamut(blob.data, blob.size);
+  }
+  return E_OK;
 }
+template int JpegRCodec::decode_batch_files(TranscodeBatchItem*, int, int, int, bool, int);   // transcode.cu
 
 int JpegRCodec::decode_batch(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller,
                              size_t group_bytes) {
@@ -868,96 +951,21 @@ int JpegRCodec::decode_batch(DecodeBatchItem* items, int n, int k, int out_ct, f
 
 int JpegRCodec::decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller) {
   const bool sdr_only = out_ct == UHDR_CT_SRGB;
-  int rc = E_OK;
-  // 1. per item, the header stages of both JPEGs (decode_body's order: primary, then map)
-  if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
-  if ((int)batch_idct_.size() < 2 * n) batch_idct_.resize(2 * n);
-  JpegBatchScan* scans = batch_scans_.data();
-  int ns = 0;
-  for (int i = 0; i < n; i++) {
-    DecodeBatchItem& it = items[i];
-    if (it.rc) continue;
-    const DecodedInfo& in = it.info;
-    const bool want_map = it.gainmap || !sdr_only;
-    it.map_rc = E_OK;
-    rc = decode_jpeg_begin(ws_, it.data + in.base_off, in.base_len, sdr_only ? 1 : 0, k, &it.sdr, &it.ph, &it.pj);
-    if (rc == E_MEM) return rc;
-    if (rc) {
-      batch_item_fail(it, rc, last_error());
-      continue;
-    }
-    scans[ns++] = JpegBatchScan{it.data + in.base_off, in.base_len, &it.ph, {}, 0, {0}};
-    if (!want_map) continue;
-    it.map_rc = decode_jpeg_begin(ws_, it.data + in.gainmap_off, in.gainmap_len, 2, k, &it.map, &it.gh, &it.gj);
-    if (it.map_rc == E_MEM) return E_MEM;
-    if (it.map_rc) snprintf(it.map_err, sizeof it.map_err, "%s", last_error());
-    else scans[ns++] = JpegBatchScan{it.data + in.gainmap_off, in.gainmap_len, &it.gh, {}, 0, {0}};
-  }
-  // 2. entropy decoding of every scan
-  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
-  // 3. in the order decode() meets them: the primary's result and its tail stage (which launches nothing for these
-  // modes), the map header's error, the map's result; then one inverse DCT for everything that is left
-  JpegIdctJob* jobs = batch_idct_.data();
-  int nj = 0, si = 0;
-  auto add_job = [&](const JpegHeader& h, const JpegDecodeJob& j, const JpegBatchScan& sc) {
-    JpegIdctJob& o = jobs[nj++];
-    o.h = &h;
-    o.g = j.k != 1 ? &j.g : nullptr;
-    for (int c = 0; c < 3; c++) {
-      o.d_coefs[c] = sc.d_coefs[c];
-      o.planes[c] = j.planes[c];
-      o.strides[c] = j.strides[c];
-    }
-  };
-  for (int i = 0; i < n; i++) {
-    DecodeBatchItem& it = items[i];
-    if (it.rc) continue;
-    const bool want_map = it.gainmap || !sdr_only;
-    const JpegBatchScan& ps = scans[si++];
-    const JpegBatchScan* gs = want_map && !it.map_rc ? &scans[si++] : nullptr;
-    if (ps.rc) {
-      batch_item_fail(it, ps.rc, ps.err);
-      continue;
-    }
-    rc = decode_jpeg_end(ws_, &it.ph, it.pj, &it.sdr, sdr_only ? &it.to_rgba : nullptr);
-    if (rc) {
-      batch_item_fail(it, rc, last_error());
-      continue;
-    }
-    if (it.map_rc) {
-      batch_item_fail(it, it.map_rc, it.map_err);
-      continue;
-    }
-    if (gs && gs->rc) {
-      batch_item_fail(it, gs->rc, gs->err);
-      continue;
-    }
-    add_job(it.ph, it.pj, ps);
-    if (gs) add_job(it.gh, it.gj, *gs);
-  }
-  if (nj && (rc = jpeg_idct_batch_dev(ws_, jobs, nj))) return rc;
-  // 4. per item: the map's tail stage, the gamuts, the metadata, then the writes into the caller's planes
+  for (int i = 0; i < n; i++) items[i].want_map = items[i].gainmap || !sdr_only;   // decode_body's want_map
+  // DECODE_TO_RGB_CS / DECODE_TO_YCBCR_CS, the SRGB colour conversion writing the caller's plane; DECODE_STREAM
+  int rc = decode_batch_files(items, n, k, sdr_only ? 1 : 0, sdr_only, 2);
+  if (rc) return rc;
+  // then per item the metadata and the writes into the caller's planes
   if ((rc = join_caller(caller))) return rc;
   for (int i = 0; i < n; i++) {
     DecodeBatchItem& it = items[i];
     if (it.rc) continue;
-    const bool want_map = it.gainmap || !sdr_only;
     const uint8_t* pd = it.data + it.info.base_off;
     const uint8_t* gd = it.data + it.info.gainmap_off;
-    ByteView blob = find_marker(pd, it.ph, 0xE2, "ICC_PROFILE", 12);
-    it.sdr.cg = icc_read_gamut(blob.data, blob.size);
     int r = E_OK;
-    if (want_map) {
-      r = decode_jpeg_end(ws_, &it.gh, it.gj, &it.map, nullptr);
-      if (r == E_MEM) return r;
-      if (!r) {
-        blob = find_marker(gd, it.gh, 0xE2, "ICC_PROFILE", 12);
-        it.map.cg = icc_read_gamut(blob.data, blob.size);
-      }
-    }
     uhdr_gainmap_metadata_t md{};
-    if (!r && (it.md_out || !sdr_only)) {  // decode_body's metadata step
-      if (!want_map) {
+    if (it.md_out || !sdr_only) {  // decode_body's metadata step
+      if (!it.want_map) {
         r = fail(E_INVALID_PARAM, "received no valid buffer to parse gainmap metadata");
       } else {
         const ByteView iso = find_marker(gd, it.gh, 0xE2, "urn:iso:std:iso:ts:21496:-1", 28);
@@ -970,7 +978,7 @@ int JpegRCodec::decode_batch_group(DecodeBatchItem* items, int n, int k, int out
     if (!r) r = check_dev_outputs(it.sdr, it.map, out_ct, it.dest, it.gainmap);
     if (!r) r = enqueue_dev_writes(it.sdr, it.map, it.to_rgba, md, out_ct, max_display_boost, it.dest, it.gainmap);
     if (r == E_MEM) return r;
-    if (r) batch_item_fail(it, r, last_error());
+    if (r) batch_fail(it, r, last_error());
   }
   return E_OK;
 }

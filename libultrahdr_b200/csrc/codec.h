@@ -3,6 +3,7 @@
 // the marker/container layer is host code.
 #pragma once
 #include <condition_variable>
+#include <cstdio>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -31,41 +32,42 @@ struct JpegDecodeJob {
   int strides[3] = {0, 0, 0};
 };
 
-// One file of JpegRCodec::decode_batch.  The caller fills the first group of fields; rc != E_OK on entry skips the item.
-struct DecodeBatchItem {
+// One JPEG/R file of a batched call (decode_batch, transcode_batch).  The caller fills the first group of fields;
+// rc != E_OK on entry skips the file.
+struct BatchFile {
   const uint8_t* data = nullptr;
   size_t size = 0;
   DecodedInfo info;  // probe() of the file
-  uhdr_raw_image_t* dest = nullptr;
-  uhdr_raw_image_t* gainmap = nullptr;
-  uhdr_gainmap_metadata_t* md_out = nullptr;
-  int rc = 0;        // out: the code decode() gives for this file alone, its message in err
+  bool want_map = true;   // the gain-map JPEG is decoded too
+  int rc = 0;        // out: the code the single call gives for this file alone, its message in err
   char err[256] = {0};
-  // the decode's state between its batched stages
+  // the two JPEGs' decode between its batched stages (JpegRCodec::decode_batch_files)
   JpegHeader ph, gh;
   JpegDecodeJob pj, gj;
   DevImage sdr{}, map{};
-  YccToRgbaParams to_rgba{};
+  YccToRgbaParams to_rgba{};   // the primary's colour conversion when decode_batch_files defers it
   int map_rc = 0;    // an error of the gain-map JPEG's header stage, returned after the primary image's own
   char map_err[256] = {0};
 };
 
-// One file of JpegRCodec::transcode_batch.  The caller fills the first group of fields; rc != E_OK on entry skips the item.
-struct TranscodeBatchItem {
-  const uint8_t* data = nullptr;
-  size_t size = 0;
-  DecodedInfo info;  // probe() of the file
+// the file's code and message: it drops out of the rest of the batch
+inline void batch_fail(BatchFile& f, int rc, const char* msg) {
+  f.rc = rc;
+  snprintf(f.err, sizeof f.err, "%s", msg);
+}
+
+// One file of JpegRCodec::decode_batch: the decode() outputs
+struct DecodeBatchItem : BatchFile {
+  uhdr_raw_image_t* dest = nullptr;
+  uhdr_raw_image_t* gainmap = nullptr;
+  uhdr_gainmap_metadata_t* md_out = nullptr;
+};
+
+// One file of JpegRCodec::transcode_batch: the transcode() output and the two encodes between their batched stages
+struct TranscodeBatchItem : BatchFile {
   uint8_t* out = nullptr;
   size_t cap = 0;
   size_t out_size = 0;  // out: what transcode() sets
-  int rc = 0;        // out: the code transcode() gives for this file alone, its message in err
-  char err[256] = {0};
-  // the transcode's state between its batched stages
-  JpegHeader ph, gh;
-  JpegDecodeJob pj, gj;
-  DevImage sdr{}, map{};
-  int map_rc = 0;    // an error of the gain-map JPEG's header stage, returned after the primary image's own
-  char map_err[256] = {0};
   JpegEncodeJob base_jpeg, gm_jpeg;
 };
 
@@ -203,6 +205,13 @@ class JpegRCodec {
   int enqueue_dev_writes(const DevImage& sdr, const DevImage& map, const YccToRgbaParams& to_rgba,
                          const uhdr_gainmap_metadata_t& md, int out_ct, float max_display_boost,
                          uhdr_raw_image_t* dest, uhdr_raw_image_t* gainmap_out);
+  // Both batched calls' decode of a group (Item: DecodeBatchItem or TranscodeBatchItem), as decode_pair would decode
+  // each file at 1/k: the headers, one entropy decoding and one inverse DCT for every scan, the tail stages and the
+  // gamuts.  sdr_mode / map_mode: decode_jpeg_dev's modes; defer_rgba: the primary's colour conversion (mode 1) is left
+  // in to_rgba.  A file's own error goes to the file, in the order the single call meets it; the return value is an
+  // error that ends the call (CUDA, memory).
+  template <class Item>
+  int decode_batch_files(Item* items, int n, int k, int sdr_mode, bool defer_rgba, int map_mode);
   int decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller);
   int transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg);
   // transcode()'s last stage, once both scans are on the host: API-4's checks, the heads, EXIF, the container, the cap

@@ -244,11 +244,6 @@ int JpegRCodec::transcode_finish(const uint8_t* data, const DecodedInfo& probed,
 
 namespace {
 
-void item_fail(TranscodeBatchItem& it, int rc, const char* msg) {
-  it.rc = rc;
-  snprintf(it.err, sizeof it.err, "%s", msg);
-}
-
 // a workspace plane of aw x rows bytes for the block stage
 int stage_plane(Workspace& ws, int aw, int rows, uint8_t** out) {
   *out = (uint8_t*)ws.dalloc((size_t)aw * rows);
@@ -365,83 +360,10 @@ int JpegRCodec::transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b20
 }
 
 int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg) {
-  const int k = cfg.k;
-  int rc = E_OK;
-  // 1. per item, the header stages of both JPEGs (decode_pair's order: primary, then map), raw planes for both
-  if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
-  if ((int)batch_idct_.size() < 2 * n) batch_idct_.resize(2 * n);
+  // 1-3. both JPEGs of every item decoded as transcode() decodes them: raw planes, a 3-channel map as YCbCr
+  int rc = decode_batch_files(items, n, cfg.k, 0, false, 0);
+  if (rc) return rc;
   if ((int)batch_enc_.size() < 2 * n) batch_enc_.resize(2 * n);
-  JpegBatchScan* scans = batch_scans_.data();
-  int ns = 0;
-  for (int i = 0; i < n; i++) {
-    TranscodeBatchItem& it = items[i];
-    if (it.rc) continue;
-    const DecodedInfo& in = it.info;
-    it.map_rc = E_OK;
-    rc = decode_jpeg_begin(ws_, it.data + in.base_off, in.base_len, 0, k, &it.sdr, &it.ph, &it.pj);
-    if (rc == E_MEM) return rc;
-    if (rc) {
-      item_fail(it, rc, last_error());
-      continue;
-    }
-    scans[ns++] = JpegBatchScan{it.data + in.base_off, in.base_len, &it.ph, {}, 0, {0}};
-    it.map_rc = decode_jpeg_begin(ws_, it.data + in.gainmap_off, in.gainmap_len, 0, k, &it.map, &it.gh, &it.gj);
-    if (it.map_rc == E_MEM) return E_MEM;
-    if (it.map_rc) snprintf(it.map_err, sizeof it.map_err, "%s", last_error());
-    else scans[ns++] = JpegBatchScan{it.data + in.gainmap_off, in.gainmap_len, &it.gh, {}, 0, {0}};
-  }
-  // 2. entropy decoding of every scan
-  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
-  // 3. in the order transcode() meets them: the primary's result and its tail stage, the map header's error, the map's
-  // result and tail stage, the 4:2:2 check of base_420; then one inverse DCT for everything that is left
-  JpegIdctJob* jobs = batch_idct_.data();
-  int nj = 0, si = 0;
-  auto add_job = [&](const JpegHeader& h, const JpegDecodeJob& j, const JpegBatchScan& sc) {
-    JpegIdctJob& o = jobs[nj++];
-    o.h = &h;
-    o.g = j.k != 1 ? &j.g : nullptr;
-    for (int c = 0; c < 3; c++) {
-      o.d_coefs[c] = sc.d_coefs[c];
-      o.planes[c] = j.planes[c];
-      o.strides[c] = j.strides[c];
-    }
-  };
-  for (int i = 0; i < n; i++) {
-    TranscodeBatchItem& it = items[i];
-    if (it.rc) continue;
-    const JpegBatchScan& ps = scans[si++];
-    const JpegBatchScan* gs = !it.map_rc ? &scans[si++] : nullptr;
-    int r = ps.rc;
-    if (r) {
-      item_fail(it, r, ps.err);
-      continue;
-    }
-    if ((r = decode_jpeg_end(ws_, &it.ph, it.pj, &it.sdr, nullptr))) {
-      if (r == E_MEM) return r;
-      item_fail(it, r, last_error());
-      continue;
-    }
-    if (it.map_rc) {
-      item_fail(it, it.map_rc, it.map_err);
-      continue;
-    }
-    if (gs->rc) {
-      item_fail(it, gs->rc, gs->err);
-      continue;
-    }
-    if ((r = decode_jpeg_end(ws_, &it.gh, it.gj, &it.map, nullptr))) {
-      if (r == E_MEM) return r;
-      item_fail(it, r, last_error());
-      continue;
-    }
-    if (cfg.base_420 && it.sdr.v.fmt == F_YUV422) {
-      item_fail(it, fail_base_422(), last_error());
-      continue;
-    }
-    add_job(it.ph, it.pj, ps);
-    add_job(it.gh, it.gj, *gs);
-  }
-  if (nj && (rc = jpeg_idct_batch_dev(ws_, jobs, nj))) return rc;
   // 4. the staging jobs and the block stage's planes of both JPEGs of every item: base quantisers 0 / 1, map's 2 / 3
   StageJob* h_stage = (StageJob*)ws_.halloc(sizeof(StageJob) * 6 * n);
   unsigned* h_stage_end = (unsigned*)ws_.halloc(sizeof(unsigned) * 6 * n);
@@ -456,6 +378,10 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
   for (int i = 0; i < n; i++) {
     TranscodeBatchItem& it = items[i];
     if (it.rc) continue;
+    if (cfg.base_420 && it.sdr.v.fmt == F_YUV422) {   // after every map error, as in transcode()
+      batch_fail(it, fail_base_422(), last_error());
+      continue;
+    }
     DevImage base_in, map_in;
     int base_rows[3], map_rows[3];
     const int nst0 = nst;
@@ -468,7 +394,7 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
     if (r == E_MEM) return r;
     if (r) {
       nst = nst0;
-      item_fail(it, r, last_error());
+      batch_fail(it, r, last_error());
       continue;
     }
     for (int j = 0; j < 2; j++) {
@@ -518,7 +444,7 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
       if (!r && j->h_scan_bytes[4])
         r = fail(E_MEM, "entropy-coded segment exceeds the %zu byte device buffer", j->scan_capacity);
     if (!r) r = transcode_finish(it.data, it.info, it.ph, it.gh, it.base_jpeg, it.gm_jpeg, cfg, it.out, it.cap, &it.out_size);
-    if (r) item_fail(it, r, last_error());
+    if (r) batch_fail(it, r, last_error());
   }
   return E_OK;
 }
