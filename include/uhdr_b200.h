@@ -327,6 +327,10 @@ UHDR_EXTERN void uhdr_b200_jpeg_encode_stats(unsigned long long out[10]);
  * the rule above over all the group's blocks; not counted in uhdr_b200_jpeg_encode_stats).  Since process start:
  * out[0] = launches, out[1] = scans they coded.  Host-side counts. */
 UHDR_EXTERN void uhdr_b200_jpeg_encode_batch_stats(unsigned long long out[2]);
+/* Per-device kernel state, made once per device on its first use and kept for the life of the process.  Since
+ * process start: out[0] = constant tables uploaded to a device (code books, log2 table, zigzag order), out[1] = wave
+ * sizes (co-resident CTAs of a kernel) asked of the CUDA runtime.  Host-side counts; needs no device. */
+UHDR_EXTERN void uhdr_b200_device_state_stats(unsigned long long out[2]);
 /* diagnostic: worst[0] = max |approximate pow(e, 1/2.4) - the exact one| over the `count` floats whose bit patterns
  * start at first_bits (the screen relies on <= 3e-7 for e in (0.0031308, 1]; must measure <= 1.5e-7); host pointer. */
 UHDR_EXTERN int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst);

@@ -21,6 +21,7 @@
 #include "kernels.cuh"
 #include "packed_f32.cuh"
 #include "powf_glibc.cuh"
+#include "runtime.h"
 #include "tables.h"
 
 namespace uhdr_b200 {
@@ -457,17 +458,11 @@ cudaError_t launch_lin1(const ApplyParams& p, const float* gain_u8, unsigned* sc
   dim3 block(kBlockX, kBlockY);
   const int g = p.gamut_identity ? 0 : (p.gamut_on_sdr ? 1 : 2);
   // persistent grid = exactly the CTAs that are co-resident (a partial second wave would double the time)
-  static int resident[3] = {0, 0, 0};
-  if (!resident[g]) {
-    int per_sm = 0, dev = 0, sms = 0;
-    const void* fn = g == 0 ? (const void*)k_apply_lin1<BPP, 0, NANS, ORG> : g == 1 ? (const void*)k_apply_lin1<BPP, 1, NANS, ORG>
-                                                                              : (const void*)k_apply_lin1<BPP, 2, NANS, ORG>;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBlockX * kBlockY, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident[g] = per_sm * (sms > 0 ? sms : 132);
-  }
-  int ctas = resident[g];
+  static PerDevice<int> wave[3];
+  const void* fn = g == 0 ? (const void*)k_apply_lin1<BPP, 0, NANS, ORG> : g == 1 ? (const void*)k_apply_lin1<BPP, 1, NANS, ORG>
+                                                                            : (const void*)k_apply_lin1<BPP, 2, NANS, ORG>;
+  int ctas = wave_ctas(wave[g], fn, kBlockX * kBlockY, 0);
+  if (!ctas) return cudaErrorUnknown;
   if (ctas > ntiles) ctas = ntiles;
   if (g == 0) k_apply_lin1<BPP, 0, NANS, ORG><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);
   else if (g == 1) k_apply_lin1<BPP, 1, NANS, ORG><<<ctas, block, 0, s>>>(p, gain_u8, tiles_x, ntiles, kNegZero2, sched);

@@ -91,6 +91,10 @@ UHDR_API void uhdr_b200_jpeg_encode_batch_stats(unsigned long long out[2]) {
   if (out) jpeg_encode_batch_stats(out);
 }
 
+UHDR_API void uhdr_b200_device_state_stats(unsigned long long out[2]) {
+  if (out) device_state_stats(out);
+}
+
 UHDR_API int uhdr_b200_probe_pow_fast(unsigned first_bits, unsigned count, float* worst) {
   Workspace* ws = tls_workspace();
   if (!ws || !worst) return E_ERROR;

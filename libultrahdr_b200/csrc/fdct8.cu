@@ -12,7 +12,6 @@
 // from one read of the pixels.
 // Arithmetic is libjpeg-turbo's jccolor.c / jfdctint.c / jcdctmgr.c integer arithmetic: bit-exact.
 #include <cstring>
-#include <mutex>
 
 #include "kernels.cuh"
 #include "runtime.h"
@@ -438,35 +437,20 @@ __global__ void __launch_bounds__(256, 4) k_fdct8_code_batch(const __grid_consta
 
 void jpeg_std_codebook(int which, uint32_t out[256]);  // jpeg_host.cpp: (code << 8 | length) per symbol
 
-// the two AC code books (luminance, chrominance), once per device
-static int fdct_device_books(const uint32_t** out) {
-  static std::mutex mu;
-  static uint32_t* per_dev[64] = {nullptr};
-  int dev = -1;
-  CUDA_TRY(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return fail(E_ERROR, "device ordinal %d out of range", dev);
-  std::lock_guard<std::mutex> lk(mu);
-  if (!per_dev[dev]) {
-    uint32_t host[512];
-    jpeg_std_codebook(1, host);
-    jpeg_std_codebook(3, host + 256);
-    uint32_t* d = nullptr;
-    CUDA_TRY(cudaMalloc(&d, sizeof host));
-    if (int rc = copy_sync(d, host, sizeof host, cudaMemcpyHostToDevice)) return rc;
-    per_dev[dev] = d;
-  }
-  *out = per_dev[dev];
-  return E_OK;
+// the two AC code books (luminance, chrominance), once per device; nullptr + last error on failure
+static const uint32_t* fdct_device_books() {
+  static PerDevice<const void*> books;
+  return (const uint32_t*)device_table(books, 2 * 256 * sizeof(uint32_t), [](void* host) {
+    jpeg_std_codebook(1, (uint32_t*)host);
+    jpeg_std_codebook(3, (uint32_t*)host + 256);
+  });
 }
 
 cudaError_t launch_fdct8(const Fdct8Params& Pin, cudaStream_t s) {
   count_launches(1);
   Fdct8Params P = Pin;
   const bool code = P.zigzag != 0;   // zigzag launches feed the device entropy coder
-  if (code) {
-    int rc = fdct_device_books(&P.acbooks);
-    if (rc) return cudaErrorUnknown;
-  }
+  if (code && !(P.acbooks = fdct_device_books())) return cudaErrorUnknown;
   for (int t = 0; t < 2; t++)
     for (int i = 0; i < 64; i++) {
       const unsigned d = (unsigned)P.q[t][i] << 3;
@@ -488,22 +472,10 @@ cudaError_t launch_fdct8(const Fdct8Params& Pin, cudaStream_t s) {
     P.tile_end[i] = total;
   }
   if (total == 0) return cudaSuccess;
-  static int resident_tab[2] = {0, 0};  // CTAs of one wave, per kernel
-  int& resident = resident_tab[code ? 1 : 0];
-  if (!resident) {
-    int per_sm = 0, dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaError_t oe;
-    if (code) {
-      cudaFuncSetAttribute(k_fdct8_code, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CodeSmem));
-      oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fdct8_code, 256, sizeof(CodeSmem));
-    } else {
-      oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fdct8<false>, 256, 0);
-    }
-    if (oe != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident = per_sm * (sms > 0 ? sms : 132);
-  }
+  static PerDevice<int> wave[2];  // k_fdct8<false>, k_fdct8_code
+  const int resident = code ? wave_ctas(wave[1], (const void*)k_fdct8_code, 256, sizeof(CodeSmem))
+                            : wave_ctas(wave[0], (const void*)k_fdct8<false>, 256, 0);
+  if (!resident) return cudaErrorUnknown;
   if (code) {
     const int need = (total + 7) / 8;
     const int ctas = need < resident ? need : resident;
@@ -525,24 +497,16 @@ cudaError_t launch_fdct8_code_batch(const Fdct8Plane* planes, const unsigned* it
   P.item_end = item_end;
   P.nplanes = nplanes;
   P.total = total_items;
-  if (fdct_device_books(&P.acbooks)) return cudaErrorUnknown;
+  if (!(P.acbooks = fdct_device_books())) return cudaErrorUnknown;
   for (int t = 0; t < 4; t++)
     for (int i = 0; i < 64; i++) {
       P.q[t][i] = q[t][i];
       const unsigned d = (unsigned)q[t][i] << 3;
       P.mag[t][i] = d ? (unsigned)((0x100000000ull + d - 1) / d) : 0u;
     }
-  static int resident = 0;  // CTAs of one wave
-  if (!resident) {
-    int per_sm = 0, dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaFuncSetAttribute(k_fdct8_code_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CodeBatchSmem));
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fdct8_code_batch, 256, sizeof(CodeBatchSmem)) != cudaSuccess ||
-        per_sm < 1)
-      per_sm = 1;
-    resident = per_sm * (sms > 0 ? sms : 132);
-  }
+  static PerDevice<int> wave;
+  const int resident = wave_ctas(wave, (const void*)k_fdct8_code_batch, 256, sizeof(CodeBatchSmem));
+  if (!resident) return cudaErrorUnknown;
   const unsigned need = (total_items + 7) / 8;
   const unsigned ctas = need < (unsigned)resident ? need : (unsigned)resident;
   k_fdct8_code_batch<<<ctas, 256, sizeof(CodeBatchSmem), s>>>(P);

@@ -29,7 +29,6 @@
 // in kMaxRounds rounds, or whose intervals do not decode to exactly their quota of blocks return
 // kHuffDecFallback and the caller uses the host decoder of jpeg_host.cpp.
 #include <atomic>
-#include <mutex>
 #include <climits>
 #include <cstring>
 
@@ -588,20 +587,10 @@ static unsigned hd_intervals(unsigned* starts, unsigned* first, unsigned nint, u
   return (unsigned)nseq_total;
 }
 
-// kZigzagDev: once per device, synchronously and under a lock (decodes run concurrently on several streams / threads)
+// kZigzagDev, once per device
 static int upload_zigzag() {
-  static std::mutex zig_mu;
-  static bool zig_done[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lk(zig_mu);
-  if (dev < 0 || dev >= 64 || !zig_done[dev]) {
-    void* zig = nullptr;
-    CUDA_TRY(cudaGetSymbolAddress(&zig, kZigzagDev));
-    if (int rc = copy_sync(zig, kZigzag, 64, cudaMemcpyHostToDevice)) return rc;
-    if (dev >= 0 && dev < 64) zig_done[dev] = true;
-  }
-  return E_OK;
+  static PerDevice<const void*> zigzag;
+  return device_table(zigzag, 64, [](void* host) { memcpy(host, kZigzag, 64); }, &kZigzagDev) ? E_OK : E_ERROR;
 }
 
 int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, const JpegHeader& h, int16_t* d_coefs[3]) {

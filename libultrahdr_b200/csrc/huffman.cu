@@ -555,21 +555,12 @@ static FastDiv fast_div(unsigned d) {
   return f;
 }
 
-static int device_books(const uint32_t** out) {
-  static thread_local int cached_dev = -1;
-  static thread_local uint32_t* cached = nullptr;
-  int dev = -1;
-  CUDA_TRY(cudaGetDevice(&dev));
-  if (cached && cached_dev == dev) { *out = cached; return E_OK; }
-  uint32_t host[1024];
-  for (int t = 0; t < 4; t++) jpeg_std_codebook(t, host + 256 * t);
-  uint32_t* d = nullptr;
-  CUDA_TRY(cudaMalloc(&d, sizeof host));
-  if (int rc = copy_sync(d, host, sizeof host, cudaMemcpyHostToDevice)) return rc;
-  cached = d;
-  cached_dev = dev;
-  *out = d;
-  return E_OK;
+// the four standard code books, once per device; nullptr + last error on failure
+static const uint32_t* device_books() {
+  static PerDevice<const void*> books;
+  return (const uint32_t*)device_table(books, 4 * 256 * sizeof(uint32_t), [](void* host) {
+    for (int t = 0; t < 4; t++) jpeg_std_codebook(t, (uint32_t*)host + 256 * t);
+  });
 }
 
 // what jpeg_entropy_dev planned: resident CTAs per wave, launches by bpt (index 1..8), launches beyond one wave
@@ -612,15 +603,6 @@ void huff_frame(const JpegEncodeJob& job, HuffFrame* out, size_t* nblocks) {
 // (ultrahdr_api.cpp:1294); a single scan can never need more than that in a valid encode
 size_t scan_cap(const JpegFrame& fr) { return ((size_t)fr.width * fr.height * 6 + 4096 + 3) / 4 * 4; }
 
-// CTAs of one wave of `kernel` on this device type
-int resident_ctas(const void* kernel) {
-  int per_sm = 0, dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kEncThreads, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
-  return per_sm * (sms > 0 ? sms : 132);
-}
-
 // blocks per thread: the smallest value for which the whole grid is resident at once
 int blocks_per_thread(size_t nblocks, int resident) {
   const int bpt = (int)((nblocks + (size_t)kEncThreads * resident - 1) / ((size_t)kEncThreads * resident));
@@ -632,15 +614,15 @@ int blocks_per_thread(size_t nblocks, int resident) {
 int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job) {
   if (!job->zigzag || !job->d_meta[0])
     return fail(E_ERROR, "internal: device entropy coder needs the zigzag forward stage and its block side information");
-  const uint32_t* books = nullptr;
-  int rc = device_books(&books);
-  if (rc) return rc;
+  const uint32_t* books = device_books();
+  if (!books) return E_ERROR;
   HuffFrame f;
   size_t nblocks = 0;
   huff_frame(*job, &f, &nblocks);
   const size_t cap = scan_cap(job->frame);
-  static int resident = 0;  // CTAs of one wave on this device type
-  if (!resident) resident = resident_ctas((const void*)k_huff_encode);
+  static PerDevice<int> wave;
+  const int resident = wave_ctas(wave, (const void*)k_huff_encode, kEncThreads, 0);
+  if (!resident) return E_ERROR;
   const int bpt = blocks_per_thread(nblocks, resident);
   f.bpt = bpt;
   const size_t chunk = (size_t)kEncThreads * bpt;
@@ -736,11 +718,11 @@ int jpeg_entropy_batch_dev(Workspace& ws, JpegEncodeJob* const* jobs, int n) {
   for (int i = 0; i < n; i++)
     if (!jobs[i]->zigzag || !jobs[i]->d_meta[0])
       return fail(E_ERROR, "internal: device entropy coder needs the zigzag forward stage and its block side information");
-  const uint32_t* books = nullptr;
-  int rc = device_books(&books);
-  if (rc) return rc;
-  static int resident = 0;  // CTAs of one wave on this device type
-  if (!resident) resident = resident_ctas((const void*)k_huff_encode_batch);
+  const uint32_t* books = device_books();
+  if (!books) return E_ERROR;
+  static PerDevice<int> wave;
+  const int resident = wave_ctas(wave, (const void*)k_huff_encode_batch, kEncThreads, 0);
+  if (!resident) return E_ERROR;
   HuffScanDesc* h_desc = (HuffScanDesc*)ws.halloc(sizeof(HuffScanDesc) * n);
   unsigned* h_end = (unsigned*)ws.halloc(sizeof(unsigned) * n);
   unsigned* h_ctl = (unsigned*)ws.halloc((size_t)64 * n);

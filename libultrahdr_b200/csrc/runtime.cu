@@ -35,6 +35,70 @@ int copy_sync(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
   return E_OK;
 }
 
+// ---- per-device kernel state --------------------------------------------------------------------
+namespace {
+std::atomic<unsigned long long> g_state_made[2];  // device tables, wave sizes
+
+// the slot's value for the current device; make(dev, &value) runs once per device, under the slot's lock (kernels
+// are launched from many host threads at once)
+template <class T, class Make>
+int per_device(PerDevice<T>& slot, T* out, Make make) {
+  int dev = -1;
+  CUDA_TRY(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= kMaxDevices) return fail(E_ERROR, "device ordinal %d out of range", dev);
+  T v = slot.v[dev].load(std::memory_order_acquire);
+  if (!v) {
+    std::lock_guard<std::mutex> lk(slot.mu);
+    v = slot.v[dev].load(std::memory_order_relaxed);
+    if (!v) {
+      if (int rc = make(dev, &v)) return rc;
+      slot.v[dev].store(v, std::memory_order_release);
+    }
+  }
+  *out = v;
+  return E_OK;
+}
+}  // namespace
+
+int wave_ctas(PerDevice<int>& slot, const void* kernel, int threads, size_t dyn_smem) {
+  int ctas = 0;
+  const int err = per_device(slot, &ctas, [&](int dev, int* out) -> int {
+    // function attributes belong to the device's context: every device needs its own opt-in
+    if (dyn_smem > (48 << 10))
+      CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem));
+    int sms = 0, per_sm = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, dyn_smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+    *out = per_sm * (sms > 0 ? sms : 132);
+    g_state_made[1].fetch_add(1, std::memory_order_relaxed);
+    return E_OK;
+  });
+  return err ? 0 : ctas;
+}
+
+const void* device_table(PerDevice<const void*>& slot, size_t bytes, void (*build)(void* host), const void* symbol) {
+  const void* table = nullptr;
+  const int err = per_device(slot, &table, [&](int, const void** out) -> int {
+    std::vector<unsigned char> host(bytes);
+    build(host.data());
+    void* d = nullptr;
+    if (symbol) CUDA_TRY(cudaGetSymbolAddress(&d, symbol));
+    else CUDA_TRY(cudaMalloc(&d, bytes));
+    if (int rc = copy_sync(d, host.data(), bytes, cudaMemcpyHostToDevice)) {
+      if (!symbol) cudaFree(d);
+      return rc;
+    }
+    *out = d;
+    g_state_made[0].fetch_add(1, std::memory_order_relaxed);
+    return E_OK;
+  });
+  return err ? nullptr : table;
+}
+
+void device_state_stats(unsigned long long out[2]) {
+  for (int i = 0; i < 2; i++) out[i] = g_state_made[i].load(std::memory_order_relaxed);
+}
+
 // ---- LUT residency ------------------------------------------------------------------------------
 static std::mutex g_lut_mu;
 static std::map<int, float*> g_luts;  // device ordinal -> device blob

@@ -7,7 +7,9 @@
 #include <cstdlib>
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <cstddef>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -34,6 +36,30 @@ int fail(int code, const char* fmt, ...);
 // cudaMemcpy from pageable memory (or device to device) may return before its DMA completes, and it is ordered
 // only against the legacy stream: kernels on the library's non-blocking streams could read the table before it.
 int copy_sync(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind);
+
+// ---- per-device kernel state ---------------------------------------------------------------------
+// Constant tables in device memory and wave sizes are made once per device, on its first use, and kept for the life
+// of the process.  A slot is constant-initialised: a function-local `static PerDevice<T>` has no init guard and makes
+// no heap call.  Looking a value up costs one cudaGetDevice and one acquire load; only the first use on a device
+// takes the slot's lock.  A device ordinal >= kMaxDevices is an error.
+constexpr int kMaxDevices = 64;
+template <class T>
+struct PerDevice {
+  std::atomic<T> v[kMaxDevices] = {};  // T{}: not made yet on that device (the initialiser keeps the slot constexpr)
+  std::mutex mu;
+};
+
+// CTAs of one full wave of `kernel` on the current device: SMs x co-resident CTAs per SM (1 when the occupancy query
+// fails).  A kernel launched with more than 48 KiB of dynamic shared memory is opted in to `dyn_smem` on each device
+// first.  Returns 0 + sets last error on failure.
+int wave_ctas(PerDevice<int>& slot, const void* kernel, int threads, size_t dyn_smem);
+// A constant table of `bytes` on the current device: build(host) fills it on the host, copy_sync uploads it.  With
+// `symbol` (a __device__ / __constant__ variable) the table is copied there; otherwise it gets its own allocation.
+// Returns the device address, or nullptr + sets last error.
+const void* device_table(PerDevice<const void*>& slot, size_t bytes, void (*build)(void* host),
+                         const void* symbol = nullptr);
+// out[0] = device tables made, out[1] = wave sizes asked of the runtime, since process start
+void device_state_stats(unsigned long long out[2]);
 
 // Device-resident LUT blob for the current device (built on first use, or installed from a
 // broadcast).  Returns nullptr + sets last error when no CUDA device is usable.

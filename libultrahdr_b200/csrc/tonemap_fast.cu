@@ -14,6 +14,7 @@
 #include <atomic>
 
 #include "powf_glibc.cuh"
+#include "runtime.h"
 #include "tables.h"
 
 namespace uhdr_b200 {
@@ -193,16 +194,11 @@ __global__ void __launch_bounds__(256, 3) k_tonemap_fast(const TonemapParams p, 
 
 template <bool LIMITED, bool GAMUT>
 cudaError_t launch_tm(const TonemapParams& p, int tiles_x, int ntiles, cudaStream_t s) {
-  static int resident = 0;
+  static PerDevice<int> wave;
   const size_t smem = 8192 * sizeof(float);
   auto fn = k_tonemap_fast<LIMITED, GAMUT>;
-  if (!resident) {
-    int per_sm = 0, dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident = per_sm * (sms > 0 ? sms : 132);
-  }
+  const int resident = wave_ctas(wave, (const void*)fn, 256, smem);
+  if (!resident) return cudaErrorUnknown;
   const int ctas = resident < ntiles ? resident : ntiles;
   unsigned long long* cnt = nullptr;
   if (cudaGetSymbolAddress((void**)&cnt, g_tm_exact_groups) != cudaSuccess) return cudaErrorUnknown;
