@@ -14,14 +14,6 @@ namespace uhdr_b200 {
 // ------------------------------------------------------------------------------------------------
 // encode
 // ------------------------------------------------------------------------------------------------
-// forward block stage + entropy coding, both on the device for every geometry (MCUs that reach past
-// the block grid included: huffman.cu codes libjpeg's dummy blocks)
-static int block_stage(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job) {
-  int rc = jpeg_forward_dev(ws, img, quality, job, /*zigzag=*/true);
-  if (rc) return rc;
-  return jpeg_entropy_dev(ws, job);
-}
-
 // The block stage loads whole 8-sample rows of 8-byte aligned blocks (fdct8.cu).  A caller's device plane is
 // read as it is only when that touches nothing past the width: 8-byte aligned rows and a plane width that is a
 // multiple of 8 (RGB888 replicates its last column instead).  Otherwise it is staged into a workspace copy with
@@ -99,24 +91,14 @@ int compress_image_dev(Workspace& ws, const DevImage& img_in, int quality, const
   DevImage img = img_in;
   int rc = caller_planes ? block_stage_input(ws, &img) : E_OK;
   if (rc) return rc;
-  JpegEncodeJob job;
-  rc = jpeg_forward_dev(ws, img, quality, &job, /*zigzag=*/true, rows);
-  if (rc) return rc;
-  rc = jpeg_entropy_dev(ws, &job);
-  if (rc) return rc;
-  rc = ws.sync();
-  if (rc) return rc;
-  rc = jpeg_entropy_fetch(ws, &job);
-  if (rc) return rc;
-  rc = ws.sync();
-  if (rc) return rc;
-  std::vector<uint8_t> s;
-  const bool gm = img.v.fmt == F_RGB888 || img.v.fmt == F_Y400;  // the reference's is_gainmap_comment
-  rc = jpeg_finish_stream(job, icc, icc_size, gm ? jpeg_gainmap_comment() : nullptr, &s);
-  if (rc) return rc;
-  if (s.size() > cap) return fail(E_MEM, "output buffer too small: need %zu bytes", s.size());
-  memcpy(out, s.data(), s.size());
-  *out_size = s.size();
+  JpegEncodeJob job, *jobs[] = {&job};
+  JpegPieces p;
+  if ((rc = jpeg_encode_dev(ws, img, quality, &job, rows)) || (rc = jpeg_entropy_collect(ws, jobs, 1)) ||
+      (rc = jpeg_stream_pieces(ws, job, icc, icc_size, &p)))
+    return rc;
+  if (p.total() > cap) return fail(E_MEM, "output buffer too small: need %zu bytes", p.total());
+  p.copy_to(out);
+  *out_size = p.total();
   return E_OK;
 }
 
@@ -147,7 +129,7 @@ int JpegRCodec::encode(const DevImage& hdr, const DevImage* sdr_in, const uhdr_b
   rc = generate_gainmap_dev(ws_, sdr, hdr, cfg, 64, &gm);
   if (rc) return rc;
   JpegEncodeJob gm_jpeg, base_jpeg;
-  rc = block_stage(ws_, gm.map, cfg.quality, &gm_jpeg);
+  rc = jpeg_encode_dev(ws_, gm.map, cfg.quality, &gm_jpeg);
   if (rc) return rc;
   // base image: icc of the sdr intent's gamut is chosen before the yuv re-encoding (:260)
   const int sdr_cg = sdr.cg;
@@ -165,16 +147,10 @@ int JpegRCodec::encode(const DevImage& hdr, const DevImage* sdr_in, const uhdr_b
     // a Display-P3 intent is still the caller's plane
     if (caller_planes && sdr.v.p[0] == sdr_in->v.p[0] && (rc = block_stage_input(ws_, &sdr))) return rc;
   }
-  rc = block_stage(ws_, sdr, base_quality, &base_jpeg);
+  rc = jpeg_encode_dev(ws_, sdr, base_quality, &base_jpeg);
   if (rc) return rc;
-  rc = ws_.sync();
-  if (rc) return rc;
-  if (gm_jpeg.h_scan_bytes || base_jpeg.h_scan_bytes) {  // sizes are known now: fetch the segments
-    if (gm_jpeg.h_scan_bytes && (rc = jpeg_entropy_fetch(ws_, &gm_jpeg))) return rc;
-    if (base_jpeg.h_scan_bytes && (rc = jpeg_entropy_fetch(ws_, &base_jpeg))) return rc;
-    rc = ws_.sync();
-    if (rc) return rc;
-  }
+  JpegEncodeJob* jobs[] = {&gm_jpeg, &base_jpeg};   // the map's overflow is the one reported
+  if ((rc = jpeg_entropy_collect(ws_, jobs, 2))) return rc;
   uhdr_gainmap_metadata_t md;
   finish_gainmap_metadata(gm, &md);
   size_t icc_gm_n = 0, icc_base_n = 0;
@@ -182,17 +158,23 @@ int JpegRCodec::encode(const DevImage& hdr, const DevImage* sdr_in, const uhdr_b
   const uint8_t* icc_base = icc_profile(UHDR_CT_SRGB, sdr_cg, &icc_base_n);
   // the two JPEG heads are written into the workspace's host arena: no heap on this path
   JpegPieces pg, pb;
-  const size_t gm_cap = jpeg_head_capacity(icc_gm_n, jpeg_gainmap_comment()), base_cap = jpeg_head_capacity(icc_base_n, nullptr);
-  uint8_t* gm_head = (uint8_t*)ws_.halloc(gm_cap);
-  uint8_t* base_head = (uint8_t*)ws_.halloc(base_cap);
-  if (!gm_head || !base_head) return E_MEM;
-  rc = jpeg_stream_pieces(gm_jpeg, icc_gm, icc_gm_n, jpeg_gainmap_comment(), gm_head, gm_cap, &pg.head_len, &pg.scan, &pg.scan_len);
-  if (rc) return rc;
-  rc = jpeg_stream_pieces(base_jpeg, icc_base, icc_base_n, nullptr, base_head, base_cap, &pb.head_len, &pb.scan, &pb.scan_len);
-  if (rc) return rc;
-  pg.head = gm_head;
-  pb.head = base_head;
+  if ((rc = jpeg_stream_pieces(ws_, gm_jpeg, icc_gm, icc_gm_n, &pg)) ||
+      (rc = jpeg_stream_pieces(ws_, base_jpeg, icc_base, icc_base_n, &pb)))
+    return rc;
   return assemble_jpegr(pb, pg, exif, exif_size, md, out, cap, out_size);
+}
+
+int api4_icc(const ByteView& base_icc, bool map_has_icc, int base_cg, const uhdr_gainmap_metadata_t& md, const uint8_t** icc,
+             size_t* icc_n) {
+  if (!md.use_base_cg && !map_has_icc)
+    return fail(E_UNSUPPORTED, "For gainmap application space to be alternate image space, gainmap image is expected to "
+                "contain alternate image color space in the form of ICC. The ICC marker in gainmap jpeg is missing.");
+  *icc = nullptr;
+  *icc_n = 0;
+  if (!base_icc.empty()) return E_OK;   // add ICC if not already present
+  if (base_cg <= UHDR_CG_UNSPECIFIED || base_cg > UHDR_CG_BT_2100) return fail(E_INVALID_PARAM, "Unrecognized 420 color gamut %d", base_cg);
+  *icc = icc_profile(UHDR_CT_SRGB, base_cg, icc_n);
+  return E_OK;
 }
 
 int JpegRCodec::encode_from_compressed(const uint8_t* base, size_t base_size, int base_cg, const uint8_t* gainmap, size_t gainmap_size,
@@ -200,26 +182,17 @@ int JpegRCodec::encode_from_compressed(const uint8_t* base, size_t base_size, in
   JpegHeader bh;
   int rc = jpeg_read_header(base, base_size, &bh);  // parseImage :392
   if (rc) return rc;
-  ByteView blob;
-  if (!md.use_base_cg) {
+  bool map_has_icc = false;
+  if (!md.use_base_cg) {   // the map is parsed only then
     JpegHeader gh;
     rc = jpeg_read_header(gainmap, gainmap_size, &gh);
     if (rc) return rc;
-    blob = find_marker(gainmap, gh, 0xE2, "ICC_PROFILE", 12);
-    if (blob.empty())
-      return fail(E_UNSUPPORTED, "For gainmap application space to be alternate image space, gainmap image is expected to "
-                  "contain alternate image color space in the form of ICC. The ICC marker in gainmap jpeg is missing.");
+    map_has_icc = !find_marker(gainmap, gh, 0xE2, "ICC_PROFILE", 12).empty();
   }
-  blob = find_marker(base, bh, 0xE2, "ICC_PROFILE", 12);
-  const uint8_t* icc = nullptr;
-  size_t icc_n = 0;
-  if (blob.empty()) {  // add ICC if not already present
-    if (base_cg <= UHDR_CG_UNSPECIFIED || base_cg > UHDR_CG_BT_2100) return fail(E_INVALID_PARAM, "Unrecognized 420 color gamut %d", base_cg);
-    icc = icc_profile(UHDR_CT_SRGB, base_cg, &icc_n);
-  }
-  JpegPieces pb, pg;
-  pb.head = base; pb.head_len = base_size; pb.scan = nullptr; pb.scan_len = 0; pb.whole = true;
-  pg.head = gainmap; pg.head_len = gainmap_size; pg.scan = nullptr; pg.scan_len = 0; pg.whole = true;
+  const uint8_t* icc;
+  size_t icc_n;
+  if ((rc = api4_icc(find_marker(base, bh, 0xE2, "ICC_PROFILE", 12), map_has_icc, base_cg, md, &icc, &icc_n))) return rc;
+  const JpegPieces pb{base, base_size, nullptr, 0, true}, pg{gainmap, gainmap_size, nullptr, 0, true};
   return assemble_jpegr(pb, pg, nullptr, 0, md, out, cap, out_size, icc, icc_n);
 }
 
@@ -261,25 +234,18 @@ int JpegRCodec::encode_with_compressed_sdr(const DevImage& hdr, const DevImage* 
   GainmapJob gm;
   rc = generate_gainmap_dev(ws_, sdr, hdr, cfg, 64, &gm);
   if (rc) return rc;
-  JpegEncodeJob gm_jpeg;
-  rc = block_stage(ws_, gm.map, cfg.quality, &gm_jpeg);
-  if (rc) return rc;
-  rc = ws_.sync();
-  if (rc) return rc;
-  if ((rc = jpeg_entropy_fetch(ws_, &gm_jpeg))) return rc;
-  rc = ws_.sync();
-  if (rc) return rc;
+  JpegEncodeJob gm_jpeg, *jobs[] = {&gm_jpeg};
+  if ((rc = jpeg_encode_dev(ws_, gm.map, cfg.quality, &gm_jpeg)) || (rc = jpeg_entropy_collect(ws_, jobs, 1))) return rc;
   uhdr_gainmap_metadata_t md;
   finish_gainmap_metadata(gm, &md);
   size_t icc_gm_n = 0;
   const uint8_t* icc_gm = icc_profile(gm.map.ct, gm.map.cg, &icc_gm_n);
-  const size_t gm_cap = jpeg_head_capacity(icc_gm_n, jpeg_gainmap_comment()) + gm_jpeg.h_scan_bytes[3] + 2;
-  uint8_t* gm_file = (uint8_t*)ws_.halloc(gm_cap);
+  JpegPieces pg;
+  if ((rc = jpeg_stream_pieces(ws_, gm_jpeg, icc_gm, icc_gm_n, &pg))) return rc;
+  uint8_t* gm_file = (uint8_t*)ws_.halloc(pg.total());
   if (!gm_file) return E_MEM;
-  size_t gm_file_n = 0;
-  rc = jpeg_finish_stream_into(gm_jpeg, icc_gm, icc_gm_n, jpeg_gainmap_comment(), gm_file, gm_cap, &gm_file_n);
-  if (rc) return rc;
-  return encode_from_compressed(sdr_jpg, sdr_jpg_size, sdr_jpg_cg, gm_file, gm_file_n, md, out, cap, out_size);
+  pg.copy_to(gm_file);
+  return encode_from_compressed(sdr_jpg, sdr_jpg_size, sdr_jpg_cg, gm_file, pg.total(), md, out, cap, out_size);
 }
 
 int JpegRCodec::encode_host(const uhdr_raw_image_t& hdr, const uhdr_raw_image_t* sdr,

@@ -276,6 +276,12 @@ int helper_padding(Workspace& ws, const uhdr_raw_image_t& caller, cudaMemcpyKind
 // first APPn marker `id` of a header whose payload starts with `sig`, as a view into the stream d
 ByteView find_marker(const uint8_t* d, const JpegHeader& h, uint8_t id, const char* sig, size_t sig_len);
 
+// API-4's ICC rules for a primary / gain-map pair (jpegr.cpp:397-428): with md.use_base_cg = 0 the map must carry an ICC
+// profile (map_has_icc), and a primary without one (base_icc empty) gets the profile of its gamut base_cg, which must be
+// a known one.  *icc / *icc_n: the profile assemble_jpegr is to add, null when the primary keeps its own.
+int api4_icc(const ByteView& base_icc, bool map_has_icc, int base_cg, const uhdr_gainmap_metadata_t& md, const uint8_t** icc,
+             size_t* icc_n);
+
 // uhdr_enc_set_raw_image's checks of one intent's descriptor (ultrahdr_api.cpp:842-1025): its code, the last error
 // set.  The planes are not dereferenced.
 int validate_raw_intent(const uhdr_raw_image_t& img, int intent);

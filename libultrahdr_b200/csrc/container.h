@@ -6,6 +6,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <cstring>
 #include <vector>
 
 #include "bytes.h"
@@ -50,6 +51,12 @@ struct JpegPieces {
   // from SOS on are copied verbatim, EOI is not implied
   bool whole = false;
   size_t total() const { return head_len + scan_len + (whole ? 0 : 2); }
+  // the stream, EOI included, into out[0, total())
+  void copy_to(uint8_t* out) const {
+    memcpy(out, head, head_len);
+    if (scan_len) memcpy(out + head_len, scan, scan_len);
+    if (!whole) memcpy(out + head_len + scan_len, "\xFF\xD9", 2);
+  }
 };
 
 // appendGainMap with UHDR_WRITE_ISO on / UHDR_WRITE_XMP off (the reference's default build).

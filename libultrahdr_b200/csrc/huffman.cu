@@ -673,15 +673,26 @@ int jpeg_entropy_dev(Workspace& ws, JpegEncodeJob* job) {
   return E_OK;
 }
 
+int jpeg_scan_check(const JpegEncodeJob& job) {
+  if (job.h_scan_bytes[4]) return fail(E_MEM, "entropy-coded segment exceeds the %zu byte device buffer", job.scan_capacity);
+  return E_OK;
+}
+
 // second phase after the sizes are on the host: fetch exactly the bytes produced
-int jpeg_entropy_fetch(Workspace& ws, JpegEncodeJob* job) {
-  const unsigned* ctl = job->h_scan_bytes;
-  if (ctl[4]) return fail(E_MEM, "entropy-coded segment exceeds the %zu byte device buffer", job->scan_capacity);
-  const unsigned n = ctl[3];
+static int jpeg_entropy_fetch(Workspace& ws, JpegEncodeJob* job) {
+  int rc = jpeg_scan_check(*job);
+  if (rc) return rc;
+  const unsigned n = job->h_scan_bytes[3];
   job->h_scan = (uint8_t*)ws.halloc(n + 64);
   if (!job->h_scan) return E_MEM;
   CUDA_TRY(cudaMemcpyAsync(job->h_scan, job->d_scan, n, cudaMemcpyDeviceToHost, ws.stream()));
   return E_OK;
+}
+
+int jpeg_entropy_collect(Workspace& ws, JpegEncodeJob* const* jobs, int n) {
+  int rc = ws.sync();   // the scans' sizes
+  for (int i = 0; !rc && i < n; i++) rc = jpeg_entropy_fetch(ws, jobs[i]);
+  return rc ? rc : ws.sync();
 }
 
 namespace {

@@ -15,12 +15,30 @@ int jpeg_forward_dev(Workspace& ws, const DevImage& img, int quality, JpegEncode
   return E_OK;
 }
 
+int jpeg_encode_dev(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, const int* rows) {
+  int rc = jpeg_forward_dev(ws, img, quality, job, /*zigzag=*/true, rows);
+  if (rc) return rc;
+  return jpeg_entropy_dev(ws, job);
+}
+
+int jpeg_stream_pieces(Workspace& ws, const JpegEncodeJob& job, const void* icc, size_t icc_size, JpegPieces* out) {
+  const size_t cap = kJpegHeadBytes + icc_size;
+  uint8_t* head = (uint8_t*)ws.halloc(cap);
+  if (!head) return E_MEM;
+  ByteSink o(head, cap);
+  jpeg_write_headers(job, icc, icc_size, o);
+  if (!o.ok()) return fail(E_ERROR, "JPEG header of %zu bytes exceeds its bound of %zu", o.size(), cap);
+  *out = JpegPieces{head, o.size(), job.h_scan, job.h_scan_bytes[3]};
+  return E_OK;
+}
+
 int jpeg_forward_plan(Workspace& ws, const DevImage& img, int quality, JpegEncodeJob* job, bool zigzag, const int* rows,
                       Fdct8Params* out) {
   int rc = jpeg_frame_init(&job->frame, img.v.fmt, img.v.w, img.v.h, quality);
   if (rc) return rc;
   const JpegFrame& f = job->frame;
   job->zigzag = zigzag;
+  job->gainmap_comment = img.v.fmt == F_RGB888 || img.v.fmt == F_Y400;
   Fdct8Params& P = *out;
   memset(&P, 0, sizeof P);
   P.zigzag = zigzag ? 1 : 0;

@@ -171,15 +171,11 @@ int JpegRCodec::transcode(const uint8_t* data, size_t size, const DecodedInfo& p
       rc = stage_tight(ws_, sdr, &base_in, base_rows);
   }
   if (!rc) rc = stage_tight(ws_, map, &map_in, map_rows);
-  if (!rc) rc = jpeg_forward_dev(ws_, base_in, cfg.base_quality, &base_jpeg, /*zigzag=*/true, base_rows);
-  if (!rc) rc = jpeg_entropy_dev(ws_, &base_jpeg);
-  if (!rc) rc = jpeg_forward_dev(ws_, map_in, cfg.gainmap_quality, &gm_jpeg, /*zigzag=*/true, map_rows);
-  if (!rc) rc = jpeg_entropy_dev(ws_, &gm_jpeg);
+  if (!rc) rc = jpeg_encode_dev(ws_, base_in, cfg.base_quality, &base_jpeg, base_rows);
+  if (!rc) rc = jpeg_encode_dev(ws_, map_in, cfg.gainmap_quality, &gm_jpeg, map_rows);
   if (!rc) tr.mark("encodes enqueued");
-  if (!rc) rc = ws_.sync();   // the two scan sizes
-  if (!rc) rc = jpeg_entropy_fetch(ws_, &base_jpeg);
-  if (!rc) rc = jpeg_entropy_fetch(ws_, &gm_jpeg);
-  if (!rc) rc = ws_.sync();
+  JpegEncodeJob* jobs[] = {&base_jpeg, &gm_jpeg};   // the base's overflow is the one reported
+  if (!rc) rc = jpeg_entropy_collect(ws_, jobs, 2);
   if (rc) {
     mark_in_flight();   // as decode(): kernels of both JPEGs may still run
     return rc;
@@ -201,31 +197,15 @@ int JpegRCodec::transcode_finish(const uint8_t* data, const DecodedInfo& probed,
   const uint8_t* gd = data + probed.gainmap_off;
   const ByteView base_icc = find_marker(pd, ph, 0xE2, "ICC_PROFILE", 12), gm_icc = find_marker(gd, gh, 0xE2, "ICC_PROFILE", 12);
   const uhdr_gainmap_metadata_t& md = probed.metadata;
-  // API-4's checks (encode_from_compressed) on the new pair
-  if (!md.use_base_cg && gm_icc.empty())
-    return fail(E_UNSUPPORTED, "For gainmap application space to be alternate image space, gainmap image is expected to "
-                "contain alternate image color space in the form of ICC. The ICC marker in gainmap jpeg is missing.");
-  const uint8_t* add_icc = nullptr;
-  size_t add_icc_n = 0;
-  if (base_icc.empty()) {
-    const int cg = icc_read_gamut(base_icc.data, base_icc.size);   // the primary image's gamut as the decode gives it
-    if (cg <= UHDR_CG_UNSPECIFIED || cg > UHDR_CG_BT_2100) return fail(E_INVALID_PARAM, "Unrecognized 420 color gamut %d", cg);
-    add_icc = icc_profile(UHDR_CT_SRGB, cg, &add_icc_n);
-  }
-  const char* base_com = base_jpeg.frame.ncomp == 1 ? jpeg_gainmap_comment() : nullptr;
-  const char* gm_com = gm_jpeg.frame.ncomp == 1 ? jpeg_gainmap_comment() : nullptr;
+  // API-4's rules on the new pair; the decode gives a primary image without ICC no gamut
+  const uint8_t* add_icc;
+  size_t add_icc_n;
+  int rc = api4_icc(base_icc, !gm_icc.empty(), UHDR_CG_UNSPECIFIED, md, &add_icc, &add_icc_n);
+  if (rc) return rc;
   JpegPieces pb, pg;
-  const size_t base_cap = jpeg_head_capacity(base_icc.size, base_com), gm_cap = jpeg_head_capacity(gm_icc.size, gm_com);
-  uint8_t* base_head = (uint8_t*)ws_.halloc(base_cap);
-  uint8_t* gm_head = (uint8_t*)ws_.halloc(gm_cap);
-  if (!base_head || !gm_head) return E_MEM;
-  int rc = jpeg_stream_pieces(base_jpeg, base_icc.data, base_icc.size, base_com, base_head, base_cap, &pb.head_len, &pb.scan,
-                              &pb.scan_len);
-  if (rc) return rc;
-  rc = jpeg_stream_pieces(gm_jpeg, gm_icc.data, gm_icc.size, gm_com, gm_head, gm_cap, &pg.head_len, &pg.scan, &pg.scan_len);
-  if (rc) return rc;
-  pb.head = base_head;
-  pg.head = gm_head;
+  if ((rc = jpeg_stream_pieces(ws_, base_jpeg, base_icc.data, base_icc.size, &pb)) ||
+      (rc = jpeg_stream_pieces(ws_, gm_jpeg, gm_icc.data, gm_icc.size, &pg)))
+    return rc;
   // keep_exif: the reference moves an EXIF segment of the base image into the container right after JFIF
   // (jpegr.cpp:1173-1217), which is where appendGainMap writes an EXIF block handed to it
   const ByteView exif = cfg.keep_exif ? probed.exif : ByteView();
@@ -439,10 +419,8 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
   for (int i = 0; i < n; i++) {
     TranscodeBatchItem& it = items[i];
     if (it.rc) continue;
-    int r = E_OK;
-    for (const JpegEncodeJob* j : {&it.base_jpeg, &it.gm_jpeg})
-      if (!r && j->h_scan_bytes[4])
-        r = fail(E_MEM, "entropy-coded segment exceeds the %zu byte device buffer", j->scan_capacity);
+    int r = jpeg_scan_check(it.base_jpeg);   // in transcode()'s order
+    if (!r) r = jpeg_scan_check(it.gm_jpeg);
     if (!r) r = transcode_finish(it.data, it.info, it.ph, it.gh, it.base_jpeg, it.gm_jpeg, cfg, it.out, it.cap, &it.out_size);
     if (r) batch_fail(it, r, last_error());
   }
