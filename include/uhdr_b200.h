@@ -277,6 +277,36 @@ typedef struct uhdr_b200_transcode_item {
 } uhdr_b200_transcode_item_t;
 UHDR_EXTERN int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n,
                                           const uhdr_b200_transcode_config_t* cfg);
+/* uhdr_b200_transcode of ONE file into a ladder of outputs in one call, each rung with its own config (a recompressed
+ * full-size copy, a 1/2 preview, 1/4 and 1/8 thumbnails, ...): both JPEGs are entropy-decoded once whatever the number
+ * of rungs, one inverse DCT pass writes every reduced size the rungs ask for, and the rungs share one staging pass, one
+ * block stage per distinct (base_quality, gainmap_quality) pair and one entropy coding, with two host waits.
+ *  - Each rung gets exactly what uhdr_b200_transcode(data, size, &rung.cfg, out, cap, &out_size) gives alone: the
+ *    same bytes, out_size and status.  Rungs may repeat a k with other qualities, base_420 or keep_exif, may be
+ *    identical, and may come in any order.
+ *  - A null data or rungs, or n outside 1..16, give UHDR_CODEC_INVALID_PARAM and touch no rung.
+ *  - A rung's own errors are the single call's, in its order of checks: a null out, a k outside {1, 2, 4, 8} or a
+ *    quality outside 0..100 (UHDR_CODEC_INVALID_PARAM, before any device work); 4:2:2 / 4:4:0 / 4:1:1 at k > 1 and
+ *    base_420 on a 4:2:2 base (UHDR_CODEC_UNSUPPORTED_FEATURE); a cap that is too small (UHDR_CODEC_MEM_ERROR with
+ *    out_size set to the size needed).  Errors of the file (a failed probe, corrupt or progressive data, no metadata,
+ *    an error of the gain-map JPEG) go to every rung that is still valid, at the point the single call meets them:
+ *    when the primary image fails only at some k, the rungs at the other k go on to the map's error or succeed.
+ *  - A failing rung writes nothing to its out; the others are unaffected.  The return value is UHDR_CODEC_OK when
+ *    every rung succeeded, else the first failing rung's code, and uhdr_b200_last_error() reads "rung <i>: <message>".
+ *    An error of the whole call (CUDA, device memory) is returned and set as the status of every rung without an error
+ *    of its own.  Without a device: UHDR_CODEC_ERROR with a CUDA message, on the call and on every valid rung.
+ *  - Input and output are HOST bytes; the call returns when every output is complete.  It runs on the calling thread's
+ *    codec for the current device and may be interleaved on one thread with uhdr_b200_transcode, _batch and the
+ *    decode calls.
+ *  - A repeated ladder of the same or a smaller shape makes no heap call. */
+typedef struct uhdr_b200_transcode_rung {
+  uhdr_b200_transcode_config_t cfg;  /* this output's k, base_quality, gainmap_quality, base_420, keep_exif */
+  void* out;                         /* host buffer for this output */
+  size_t cap;
+  size_t out_size;                   /* out: bytes written; with UHDR_CODEC_MEM_ERROR, the size needed */
+  int status;                        /* out: this rung's uhdr_codec_err_t */
+} uhdr_b200_transcode_rung_t;
+UHDR_EXTERN int uhdr_b200_transcode_ladder(const void* data, size_t size, uhdr_b200_transcode_rung_t* rungs, int n);
 
 /* Measurement hooks.  Kernel timing brackets every kernel launch with CUDA events on the
  * launching stream and accumulates per-kernel totals ("name count total_ms min_ms max_ms" lines).

@@ -392,8 +392,9 @@ Item* batch_items(int n) {
 
 // The batched entry points' tail: run(group bytes) unless `rc` (dev_codec's code) already ends the call, that call-level
 // error given to every item without one of its own, each item's status, and the first failing item's code and message
+// ("<what> <index>: ")
 template <class In, class Item, class Run>
-int run_batch(In* items, Item* its, int n, int rc, Run run) {
+int run_batch(In* items, Item* its, int n, int rc, Run run, const char* what = "item") {
   if (!rc) {
     size_t group = size_t(4) << 30;
     if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
@@ -408,7 +409,7 @@ int run_batch(In* items, Item* its, int n, int rc, Run run) {
     if (b.rc && first < 0) first = i;
   }
   if (first < 0) return E_OK;
-  return fail(its[first].rc, "item %d: %s", first, its[first].err);
+  return fail(its[first].rc, "%s %d: %s", what, first, its[first].err);
 }
 }  // namespace
 
@@ -632,6 +633,51 @@ UHDR_API int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n,
   const int rc = run_batch(items, its, n, dev_codec(&c), [&](size_t group) { return c->transcode_batch(its, n, *cfg, group); });
   // out_size: bytes written, or with UHDR_CODEC_MEM_ERROR the size needed (0 when the file was not assembled)
   for (int i = 0; i < n; i++) items[i].out_size = !its[i].rc || its[i].rc == E_MEM ? its[i].out_size : 0;
+  return rc;
+}
+
+UHDR_API int uhdr_b200_transcode_ladder(const void* data, size_t size, uhdr_b200_transcode_rung_t* rungs, int n) {
+  if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed img->data field");
+  if (!rungs) return fail(E_INVALID_PARAM, "received nullptr for the rungs");
+  if (n < 1 || n > kLadderMaxRungs) return fail(E_INVALID_PARAM, "received %d rungs, expects 1 to %d", n, kLadderMaxRungs);
+  TranscodeBatchItem* its = batch_items<TranscodeBatchItem>(n);
+  bool any = false;
+  for (int i = 0; i < n; i++) {
+    const uhdr_b200_transcode_rung_t& in = rungs[i];
+    const uhdr_b200_transcode_config_t& cfg = in.cfg;
+    TranscodeBatchItem& b = its[i];
+    b.data = (const uint8_t*)data;
+    b.size = size;
+    b.cfg = cfg;
+    b.out = (uint8_t*)in.out;
+    b.cap = in.cap;
+    b.out_size = 0;
+    // uhdr_b200_transcode's argument checks, in its order
+    b.rc = !in.out ? fail(E_INVALID_PARAM, "received nullptr for the output buffer")
+           : !valid_scale(cfg.k) ? fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", cfg.k)
+           : cfg.base_quality < 0 || cfg.base_quality > 100 || cfg.gainmap_quality < 0 || cfg.gainmap_quality > 100
+               ? fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", cfg.base_quality,
+                      cfg.gainmap_quality)
+               : E_OK;
+    if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
+    any |= !b.rc;
+  }
+  // then the file's probe, host only: its error goes to every rung still valid
+  DecodedInfo info;
+  if (any) {
+    if (const int prc = JpegRCodec().probe((const uint8_t*)data, size, &info)) {
+      const std::string msg = last_error();
+      for (int i = 0; i < n; i++)
+        if (!its[i].rc) batch_fail(its[i], prc, msg.c_str());
+      any = false;
+    }
+  }
+  for (int i = 0; i < n; i++) its[i].info = info;
+  JpegRCodec* c = nullptr;
+  const int rc = run_batch(rungs, its, n, any ? dev_codec(&c) : E_OK, [&](size_t) {
+    return any ? c->transcode_ladder((const uint8_t*)data, info, its, n) : E_OK;
+  }, "rung");
+  for (int i = 0; i < n; i++) rungs[i].out_size = !its[i].rc || its[i].rc == E_MEM ? its[i].out_size : 0;
   return rc;
 }
 

@@ -373,9 +373,14 @@ int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, int mode,
   if (rc) return rc;
   rc = validate_header(*h);
   if (rc) return rc;
-  const JpegFrame& f = h->frame;
+  return decode_jpeg_plan(ws, *h, mode, k, out, j);
+}
+
+int decode_jpeg_plan(Workspace& ws, const JpegHeader& h, int mode, int k, DevImage* out, JpegDecodeJob* j) {
+  int rc = E_OK;
+  const JpegFrame& f = h.frame;
   if (mode == 2) mode = f.ncomp == 1 ? 0 : 1;  // DECODE_STREAM :344-346
-  if (h->adobe_transform == 0 && f.ncomp == 3)
+  if (h.adobe_transform == 0 && f.ncomp == 3)
     return fail(E_UNSUPPORTED, "RGB (Adobe transform 0) JPEG input is not supported by the CUDA decoder");
   if (mode == 1 && f.ncomp == 1) return fail(E_ERROR, "expected input color space to be JCS_YCbCr or JCS_RGB but got %d", 1);
   // reduced size (k > 1): every component must come out of the IDCT at the output size; other samplings would
@@ -898,6 +903,135 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
   return E_OK;
 }
 template int JpegRCodec::decode_batch_files(TranscodeBatchItem*, int, int, int, bool, int);   // transcode.cu
+
+int JpegRCodec::decode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n) {
+  // one distinct k of the ladder: both JPEGs' plans at 1/k, and the code transcode() gives at that k once decoded
+  struct LadderK {
+    int k, rc, map_rc;
+    char err[256], map_err[256];
+    JpegDecodeJob pj, gj;
+    DevImage sdr, map;
+  } ks[4];
+  int nk = 0;
+  for (int i = 0; i < n; i++) {
+    if (rungs[i].rc) continue;
+    int j = 0;
+    while (j < nk && ks[j].k != rungs[i].cfg.k) j++;
+    if (j == nk) ks[nk++].k = rungs[i].cfg.k;
+  }
+  if (!nk) return E_OK;
+  // 1. both headers once (probe() has read and checked them), then per k the plans in decode_pair's order: the primary,
+  // then the map -- whose error transcode() meets only after the primary's entropy decoding and tail stage
+  const uint8_t* pd = data + info.base_off;
+  const uint8_t* gd = data + info.gainmap_off;
+  JpegHeader ph, gh;
+  int rc = jpeg_read_header(pd, info.base_len, &ph);
+  if (!rc) rc = validate_header(ph);
+  if (rc) {
+    for (int i = 0; i < n; i++)
+      if (!rungs[i].rc) batch_fail(rungs[i], rc, last_error());
+    return E_OK;
+  }
+  int grc = jpeg_read_header(gd, info.gainmap_len, &gh);
+  if (!grc) grc = validate_header(gh);
+  char gerr[256];
+  snprintf(gerr, sizeof gerr, "%s", grc ? last_error() : "");
+  bool need_p = false, need_g = false;
+  for (int j = 0; j < nk; j++) {
+    LadderK& K = ks[j];
+    K.map_rc = E_OK;
+    K.rc = decode_jpeg_plan(ws_, ph, 0, K.k, &K.sdr, &K.pj);
+    if (K.rc == E_MEM) return E_MEM;
+    if (K.rc) {
+      snprintf(K.err, sizeof K.err, "%s", last_error());
+      continue;
+    }
+    need_p = true;
+    K.map_rc = grc ? grc : decode_jpeg_plan(ws_, gh, 0, K.k, &K.map, &K.gj);
+    if (K.map_rc == E_MEM) return E_MEM;
+    if (K.map_rc) snprintf(K.map_err, sizeof K.map_err, "%s", grc ? gerr : last_error());
+    else need_g = true;
+  }
+  // 2. one entropy decoding of each scan some k needs (a scan the device decoder declines goes to the host decoder)
+  if ((int)batch_scans_.size() < 2) batch_scans_.resize(2);
+  JpegBatchScan* scans = batch_scans_.data();
+  int ns = 0;
+  if (need_p) scans[ns++] = JpegBatchScan{pd, info.base_len, &ph, {}, 0, {0}};
+  if (need_g) scans[ns++] = JpegBatchScan{gd, info.gainmap_len, &gh, {}, 0, {0}};
+  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
+  const JpegBatchScan* ps = &scans[0];
+  const JpegBatchScan* gs = need_g ? &scans[1] : nullptr;
+  // 3. per k in transcode()'s order: the primary's scan and tail stage, the map's plan, scan and tail stage (mode 0
+  // launches nothing there); then one k_idct_multi over both JPEGs at every k left
+  auto fail_k = [](LadderK& K, int r, const char* msg) {
+    K.rc = r;
+    snprintf(K.err, sizeof K.err, "%s", msg);
+  };
+  for (int j = 0; j < nk; j++) {
+    LadderK& K = ks[j];
+    if (K.rc) continue;
+    int r = E_OK;
+    if (ps->rc) {
+      fail_k(K, ps->rc, ps->err);
+    } else if ((r = decode_jpeg_end(ws_, &ph, K.pj, &K.sdr, nullptr))) {
+      if (r == E_MEM) return r;
+      fail_k(K, r, last_error());
+    } else if (K.map_rc) {
+      fail_k(K, K.map_rc, K.map_err);
+    } else if (gs->rc) {
+      fail_k(K, gs->rc, gs->err);
+    } else if ((r = decode_jpeg_end(ws_, &gh, K.gj, &K.map, nullptr))) {
+      if (r == E_MEM) return r;
+      fail_k(K, r, last_error());
+    }
+  }
+  IdctMultiPlane* pl = (IdctMultiPlane*)ws_.halloc(sizeof(IdctMultiPlane) * 6);
+  if (!pl) return E_MEM;
+  int np = 0;
+  for (int m = 0; m < 2; m++) {
+    const JpegHeader& h = m ? gh : ph;
+    const JpegFrame& f = h.frame;
+    for (int c = 0; c < f.ncomp; c++) {
+      IdctMultiPlane& P = pl[np];
+      memset(&P, 0, sizeof P);
+      const JpegComp& comp = f.comp[c];
+      memcpy(P.q, f.qt[comp.tq], sizeof P.q);
+      P.wblocks = comp.wblocks;
+      P.blocks = comp.wblocks * comp.hblocks;
+      for (int j = 0; j < nk; j++) {
+        const LadderK& K = ks[j];
+        if (K.rc) continue;
+        const JpegDecodeJob& job = m ? K.gj : K.pj;
+        IdctMultiPlane::Out& o = P.out[P.nout++];
+        o.s = K.k == 1 ? 8 : job.g.s[c];
+        o.dst = job.planes[c];
+        o.dst_stride = job.strides[c];
+        o.dst_w = o.s == 8 ? std::min(comp.wblocks * 8, o.dst_stride) : comp.wblocks * o.s;
+        o.dst_h = comp.hblocks * o.s;
+      }
+      if (!P.nout) break;   // no k is left
+      P.coefs = (m ? gs : ps)->d_coefs[c];
+      np++;
+    }
+  }
+  if (np && (rc = jpeg_idct_multi_dev(ws_, pl, np))) return rc;
+  // 4. every rung: its k's code, or that k's decoded pair
+  for (int i = 0; i < n; i++) {
+    TranscodeBatchItem& r = rungs[i];
+    if (r.rc) continue;
+    int j = 0;
+    while (ks[j].k != r.cfg.k) j++;
+    if (ks[j].rc) {
+      batch_fail(r, ks[j].rc, ks[j].err);
+      continue;
+    }
+    r.ph = ph;
+    r.gh = gh;
+    r.sdr = ks[j].sdr;
+    r.map = ks[j].map;
+  }
+  return E_OK;
+}
 
 int JpegRCodec::decode_batch(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller,
                              size_t group_bytes) {

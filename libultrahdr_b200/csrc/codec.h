@@ -63,8 +63,10 @@ struct DecodeBatchItem : BatchFile {
   uhdr_gainmap_metadata_t* md_out = nullptr;
 };
 
-// One file of JpegRCodec::transcode_batch: the transcode() output and the two encodes between their batched stages
+// One output of JpegRCodec::transcode_batch (a file) or transcode_ladder (a rung): the transcode() settings and output,
+// and the two encodes between their batched stages
 struct TranscodeBatchItem : BatchFile {
+  uhdr_b200_transcode_config_t cfg{};
   uint8_t* out = nullptr;
   size_t cap = 0;
   size_t out_size = 0;  // out: what transcode() sets
@@ -76,6 +78,11 @@ struct TranscodeBatchItem : BatchFile {
 int decode_jpeg_begin(Workspace& ws, const uint8_t* data, size_t size, int mode, int k, DevImage* out, JpegHeader* h,
                       JpegDecodeJob* j);
 int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, DevImage* out, YccToRgbaParams* to_rgba);
+// decode_jpeg_begin's part after the header: the checks and output planes of a decode at 1/k
+int decode_jpeg_plan(Workspace& ws, const JpegHeader& h, int mode, int k, DevImage* out, JpegDecodeJob* j);
+
+// the most rungs one transcode_ladder call takes: it bounds the host plan and the scratch of one call
+constexpr int kLadderMaxRungs = 16;
 
 // One parked host thread per codec (spawned on first use, kept until the codec dies): runs the gain-map JPEG of a
 // decode next to the primary one without creating a thread per call.
@@ -176,6 +183,12 @@ class JpegRCodec {
   // and two host waits for the encoder.  Each item gets the bytes, size and code transcode() gives for it alone; a
   // failing item writes nothing.  The return value is an error that ends the whole call (CUDA, memory).
   int transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg, size_t group_bytes);
+  // transcode() of one file (`data`, `info` its probe()) into n <= kLadderMaxRungs outputs, each with its own cfg: both
+  // JPEGs entropy-decoded once, one k_idct_multi launch for every k the rungs ask for, then the batch's encode
+  // (transcode_encode).  rungs[i].rc != E_OK on entry skips the rung.  Each rung gets the bytes, size and code
+  // transcode() gives for its cfg alone; a failing rung writes nothing.  The return value is an error that ends the
+  // whole call (CUDA, memory).
+  int transcode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n);
   ~JpegRCodec();
 
  private:
@@ -214,6 +227,14 @@ class JpegRCodec {
   int decode_batch_files(Item* items, int n, int k, int sdr_mode, bool defer_rgba, int map_mode);
   int decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller);
   int transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg);
+  // transcode_ladder's decode: the headers once, per distinct k the plans of both JPEGs, one entropy decoding of each
+  // scan, the errors in transcode()'s order per k, one k_idct_multi; then each rung's decoded pair (sdr, map, ph, gh)
+  int decode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n);
+  // Both transcode paths' encode, once every item's pair is decoded: per item its cfg's 4:2:2 check of base_420, one
+  // k_stage_batch launch, one k_fdct8_code_batch launch per distinct (base_quality, gainmap_quality) pair (at most
+  // kLadderMaxRungs of them), one k_huff_encode_batch, two host waits with k_pack_scans, then per item the scan checks
+  // and transcode_finish.  A failing item gets its code; the return value is an error that ends the call.
+  int transcode_encode(TranscodeBatchItem* items, int n);
   // transcode()'s last stage, once both scans are on the host: API-4's checks, the heads, EXIF, the container, the cap
   int transcode_finish(const uint8_t* data, const DecodedInfo& probed, const JpegHeader& ph, const JpegHeader& gh,
                        const JpegEncodeJob& base_jpeg, const JpegEncodeJob& gm_jpeg, const uhdr_b200_transcode_config_t& cfg,

@@ -154,6 +154,9 @@ struct JpegIdctJob {
 };
 // The bytes jpeg_idct_dev / jpeg_idct_scaled_dev write for each job, with one launch per DCT scaled size for all of them
 int jpeg_idct_batch_dev(Workspace& ws, const JpegIdctJob* jobs, int n);
+// One launch of k_idct_multi over `planes` (host memory, n entries, copied to the device on ws.stream()): each plane's
+// coefficients are read once and written at every size its outputs ask for
+int jpeg_idct_multi_dev(Workspace& ws, const IdctMultiPlane* planes, int n);
 // Same, coefficients decoded on the host.
 int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const h_coefs[3],
                             uint8_t* d_planes[3], int plane_stride[3]);

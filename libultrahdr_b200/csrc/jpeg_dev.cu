@@ -223,6 +223,23 @@ int jpeg_idct_batch_dev(Workspace& ws, const JpegIdctJob* jobs, int n) {
   return E_OK;
 }
 
+int jpeg_idct_multi_dev(Workspace& ws, const IdctMultiPlane* planes, int n) {
+  unsigned* h_end = (unsigned*)ws.halloc(sizeof(unsigned) * n);
+  if (!h_end) return E_MEM;
+  unsigned ctas = 0;
+  for (int i = 0; i < n; i++) {
+    ctas += (unsigned)(planes[i].blocks + 127) / 128;
+    h_end[i] = ctas;
+  }
+  IdctMultiPlane* d_pl = (IdctMultiPlane*)ws.dalloc(sizeof(IdctMultiPlane) * n);
+  unsigned* d_end = (unsigned*)ws.dalloc(sizeof(unsigned) * n);
+  if (!d_pl || !d_end) return E_MEM;
+  CUDA_TRY(cudaMemcpyAsync(d_pl, planes, sizeof(IdctMultiPlane) * n, cudaMemcpyHostToDevice, ws.stream()));
+  CUDA_TRY(cudaMemcpyAsync(d_end, h_end, sizeof(unsigned) * n, cudaMemcpyHostToDevice, ws.stream()));
+  TIMED(ws, "idct_multi", launch_idct_multi(d_pl, d_end, (unsigned)n, ctas, ws.stream()));
+  return E_OK;
+}
+
 namespace {
 std::atomic<int> g_entropy_decoder{0};
 }

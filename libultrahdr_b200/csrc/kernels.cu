@@ -7,6 +7,7 @@
 
 #include <atomic>
 
+#include "idct_block.cuh"
 #include "powf_glibc.cuh"
 #include "tables.h"
 
@@ -719,107 +720,8 @@ __global__ void __launch_bounds__(256) k_yuv_convert(const YuvConvParams p) {
 // PASS1_BITS 2), jcdctmgr.c quantiser (divisor 8*Q, round half away from zero), jccolor.c /
 // jdcolor.c colour conversion.  Integer arithmetic, bit-exact.
 // ------------------------------------------------------------------------------------------------
-#define C_BITS 13
-#define P1_BITS 2
-#define FX_0_298631336 2446
-#define FX_0_390180644 3196
-#define FX_0_541196100 4433
-#define FX_0_765366865 6270
-#define FX_0_899976223 7373
-#define FX_1_175875602 9633
-#define FX_1_501321110 12299
-#define FX_1_847759065 15137
-#define FX_1_961570560 16069
-#define FX_2_053119869 16819
-#define FX_2_562915447 20995
-#define FX_3_072711026 25172
-#define DESCALE(x, n) (((x) + (1 << ((n)-1))) >> (n))
 
-// (the forward block stage lives in fdct8.cu)
-
-__device__ __forceinline__ void idct8(int d0, int d1, int d2, int d3, int d4, int d5, int d6, int d7,
-                                      int o[8], int shift) {
-  int z2 = d2, z3 = d6;
-  int z1 = (z2 + z3) * FX_0_541196100;
-  int tmp2 = z1 + z3 * (-FX_1_847759065);
-  int tmp3 = z1 + z2 * FX_0_765366865;
-  int tmp0 = (d0 + d4) << C_BITS;
-  int tmp1 = (d0 - d4) << C_BITS;
-  int tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
-  tmp0 = d7; tmp1 = d5; tmp2 = d3; tmp3 = d1;
-  z1 = tmp0 + tmp3;
-  z2 = tmp1 + tmp2;
-  z3 = tmp0 + tmp2;
-  int z4 = tmp1 + tmp3;
-  int z5 = (z3 + z4) * FX_1_175875602;
-  tmp0 *= FX_0_298631336;
-  tmp1 *= FX_2_053119869;
-  tmp2 *= FX_3_072711026;
-  tmp3 *= FX_1_501321110;
-  z1 *= -FX_0_899976223;
-  z2 *= -FX_2_562915447;
-  z3 *= -FX_1_961570560;
-  z4 *= -FX_0_390180644;
-  z3 += z5;
-  z4 += z5;
-  tmp0 += z1 + z3;
-  tmp1 += z2 + z4;
-  tmp2 += z2 + z3;
-  tmp3 += z1 + z4;
-  o[0] = DESCALE(tmp10 + tmp3, shift);
-  o[7] = DESCALE(tmp10 - tmp3, shift);
-  o[1] = DESCALE(tmp11 + tmp2, shift);
-  o[6] = DESCALE(tmp11 - tmp2, shift);
-  o[2] = DESCALE(tmp12 + tmp1, shift);
-  o[5] = DESCALE(tmp12 - tmp1, shift);
-  o[3] = DESCALE(tmp13 + tmp0, shift);
-  o[4] = DESCALE(tmp13 - tmp0, shift);
-}
-
-// block (bx, by) of a plane, quantiser in shared memory
-__device__ __forceinline__ void idct_dequant_block(const int16_t* coefs, const uint16_t* sq, int wblocks, int bx, int by, uint8_t* dst,
-                                                   int dst_stride, int dst_w, int dst_h) {
-  const int16_t* in = coefs + ((size_t)by * wblocks + bx) * 64;
-  int v[64];
-#pragma unroll
-  for (int i = 0; i < 64; i += 8) {
-    const uint4 q = __ldg((const uint4*)(in + i));
-    const unsigned w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      const int c = (int)(int16_t)((w[k >> 1] >> ((k & 1) * 16)) & 0xffff);
-      v[i + k] = c * (int)sq[i + k];
-    }
-  }
-  int o[8];
-#pragma unroll
-  for (int c = 0; c < 8; c++) {  // pass 1: columns
-    idct8(v[c], v[8 + c], v[16 + c], v[24 + c], v[32 + c], v[40 + c], v[48 + c], v[56 + c], o,
-          C_BITS - P1_BITS);
-#pragma unroll
-    for (int r = 0; r < 8; r++) v[r * 8 + c] = o[r];
-  }
-#pragma unroll
-  for (int r = 0; r < 8; r++) {  // pass 2: rows, +128, clamp (SIMD saturating pack semantics)
-    idct8(v[r * 8], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3], v[r * 8 + 4], v[r * 8 + 5],
-          v[r * 8 + 6], v[r * 8 + 7], o, C_BITS + P1_BITS + 3);
-    const int y = by * 8 + r;
-    if (y >= dst_h) continue;
-    unsigned lo = 0, hi = 0;
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-      lo |= (unsigned)min(max(o[c] + 128, 0), 255) << (8 * c);
-      hi |= (unsigned)min(max(o[4 + c] + 128, 0), 255) << (8 * c);
-    }
-    uint8_t* d = dst + (size_t)y * dst_stride + bx * 8;
-    if (bx * 8 + 8 <= dst_w && ((((size_t)d) & 7) == 0)) {
-      *(uint2*)d = make_uint2(lo, hi);
-    } else {
-      for (int c = 0; c < 8 && bx * 8 + c < dst_w; c++)
-        d[c] = (uint8_t)(((c < 4 ? lo : hi) >> (8 * (c & 3))) & 0xff);
-    }
-  }
-}
+// (the forward block stage lives in fdct8.cu, the inverse DCT's block bodies in idct_block.cuh)
 
 __global__ void __launch_bounds__(128) k_idct_dequant(const IdctPlaneParams p) {
   const int bx = blockIdx.x * blockDim.x + threadIdx.x;

@@ -179,6 +179,18 @@ struct IdctBatchPlane {
   int dst_stride;
   int dst_w, dst_h;                 // samples beyond are not written
 };
+// one plane of k_idct_multi: its coefficients decoded once, written at up to four DCT scaled sizes (the sizes a ladder of
+// 1/k decodes needs); out[i] gets the bytes k_idct_dequant (s = 8) or k_idct_scaled<s> writes for that plane
+struct IdctMultiPlane {
+  const int16_t* coefs;
+  uint16_t q[64];
+  int wblocks, blocks, nout;
+  struct Out {
+    uint8_t* dst;
+    int s, dst_stride;
+    int dst_w, dst_h;               // samples beyond are not written
+  } out[4];
+};
 // first j < n with x < end[j] (end ascending): the plane of CTA x, given each plane's last CTA + 1
 __device__ __forceinline__ unsigned batch_find(const unsigned* __restrict__ end, unsigned n, unsigned x) {
   unsigned a = 0, b = n - 1;
@@ -249,6 +261,8 @@ cudaError_t launch_idct_scaled(const IdctScaledParams& p, int size, cudaStream_t
 cudaError_t launch_idct_dequant_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s);
 cudaError_t launch_idct_scaled_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, int size,
                                      cudaStream_t s);
+// k_idct_multi: planes / cta_end as for launch_idct_dequant_batch, every output of every plane in one launch
+cudaError_t launch_idct_multi(const IdctMultiPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s);
 cudaError_t launch_ycc_to_rgba(const YccToRgbaParams& p, cudaStream_t s);
 
 // number of kernel launches issued by this library since load (bench.py's gpu_launches)

@@ -343,21 +343,40 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
   // 1-3. both JPEGs of every item decoded as transcode() decodes them: raw planes, a 3-channel map as YCbCr
   int rc = decode_batch_files(items, n, cfg.k, 0, false, 0);
   if (rc) return rc;
+  for (int i = 0; i < n; i++) items[i].cfg = cfg;
+  return transcode_encode(items, n);
+}
+
+int JpegRCodec::transcode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n) {
+  int rc = settle();
+  if (rc) return rc;
+  ws_.rewind();
+  map_pending_ = false;
+  rc = decode_ladder(data, info, rungs, n);
+  if (!rc) rc = transcode_encode(rungs, n);
+  if (rc) mark_in_flight();   // as transcode(): kernels of the call may still run
+  return rc;
+}
+
+int JpegRCodec::transcode_encode(TranscodeBatchItem* items, int n) {
   if ((int)batch_enc_.size() < 2 * n) batch_enc_.resize(2 * n);
-  // 4. the staging jobs and the block stage's planes of both JPEGs of every item: base quantisers 0 / 1, map's 2 / 3
+  // 4. the staging jobs and the block stage's planes of both JPEGs of every item; per quality pair, base quantisers
+  // 0 / 1, map's 2 / 3
   StageJob* h_stage = (StageJob*)ws_.halloc(sizeof(StageJob) * 6 * n);
   unsigned* h_stage_end = (unsigned*)ws_.halloc(sizeof(unsigned) * 6 * n);
   Fdct8Plane* h_pl = (Fdct8Plane*)ws_.halloc(sizeof(Fdct8Plane) * 6 * n);
-  unsigned* h_pl_end = (unsigned*)ws_.halloc(sizeof(unsigned) * 6 * n);
-  if (!h_stage || !h_stage_end || !h_pl || !h_pl_end) return E_MEM;
-  uint16_t q[4][64];
-  memset(q, 0, sizeof q);
-  int nst = 0, npl = 0, nenc = 0;
-  unsigned items_total = 0;
+  int* h_pair = (int*)ws_.halloc(sizeof(int) * 6 * n);
+  Fdct8Plane* h_sub = (Fdct8Plane*)ws_.halloc(sizeof(Fdct8Plane) * 6 * n);
+  unsigned* h_sub_end = (unsigned*)ws_.halloc(sizeof(unsigned) * 6 * n);
+  if (!h_stage || !h_stage_end || !h_pl || !h_pair || !h_sub || !h_sub_end) return E_MEM;
+  int pairs[kLadderMaxRungs][2], npairs = 0;
+  uint16_t q[kLadderMaxRungs][4][64];
+  int rc = E_OK, nst = 0, npl = 0, nenc = 0;
   JpegEncodeJob** enc = batch_enc_.data();
   for (int i = 0; i < n; i++) {
     TranscodeBatchItem& it = items[i];
     if (it.rc) continue;
+    const uhdr_b200_transcode_config_t& cfg = it.cfg;
     if (cfg.base_420 && it.sdr.v.fmt == F_YUV422) {   // after every map error, as in transcode()
       batch_fail(it, fail_base_422(), last_error());
       continue;
@@ -377,14 +396,20 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
       batch_fail(it, r, last_error());
       continue;
     }
+    int pi = 0;
+    while (pi < npairs && (pairs[pi][0] != cfg.base_quality || pairs[pi][1] != cfg.gainmap_quality)) pi++;
+    if (pi == npairs) {
+      if (npairs == kLadderMaxRungs) return fail(E_ERROR, "internal: more than %d quality pairs in one call", kLadderMaxRungs);
+      pairs[pi][0] = cfg.base_quality;
+      pairs[pi][1] = cfg.gainmap_quality;
+      for (int j = 0; j < 2; j++) memcpy(q[pi][2 * j], P[j].q, sizeof P[j].q);
+      npairs++;
+    }
     for (int j = 0; j < 2; j++) {
-      memcpy(q[2 * j], P[j].q, sizeof P[j].q);
       for (int c = 0; c < P[j].nplanes; c++) {
-        Fdct8Plane& pl = h_pl[npl];
-        pl = P[j].plane[c];
-        pl.tq[0] += 2 * j;
-        items_total += (unsigned)(pl.wblocks * pl.hblocks + 31) / 32;
-        h_pl_end[npl++] = items_total;
+        h_pl[npl] = P[j].plane[c];
+        h_pl[npl].tq[0] += 2 * j;
+        h_pair[npl++] = pi;
       }
     }
     enc[nenc++] = &it.base_jpeg;
@@ -397,19 +422,30 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
     ctas += (unsigned)(((size_t)J.width * (J.ycc420 ? J.p.ch : J.rows) + 255) / 256);
     h_stage_end[j] = ctas;
   }
-  // 5. one staging launch, one block-stage launch, one entropy-coding launch for the whole group
+  // 5. one staging launch, one block-stage launch per quality pair, one entropy-coding launch for every item
   StageJob* d_stage;
-  unsigned *d_stage_end, *d_pl_end;
-  Fdct8Plane* d_pl;
-  if ((rc = upload_plan(ws_, h_stage, nst, &d_stage)) || (rc = upload_plan(ws_, h_stage_end, nst, &d_stage_end)) ||
-      (rc = upload_plan(ws_, h_pl, npl, &d_pl)) || (rc = upload_plan(ws_, h_pl_end, npl, &d_pl_end)))
-    return rc;
+  unsigned* d_stage_end;
+  if ((rc = upload_plan(ws_, h_stage, nst, &d_stage)) || (rc = upload_plan(ws_, h_stage_end, nst, &d_stage_end))) return rc;
   count_launches(1);
   ws_.t_begin("stage_batch");
   k_stage_batch<<<ctas, 256, 0, ws_.stream()>>>(d_stage, d_stage_end, (unsigned)nst);
   ws_.t_end();
   CUDA_TRY(cudaGetLastError());
-  TIMED(ws_, "fdct_code_batch", launch_fdct8_code_batch(d_pl, d_pl_end, (unsigned)npl, items_total, q, ws_.stream()));
+  for (int pi = 0, off = 0; pi < npairs; pi++) {
+    int ns = 0;
+    unsigned items_total = 0;
+    for (int j = 0; j < npl; j++) {
+      if (h_pair[j] != pi) continue;
+      h_sub[off + ns] = h_pl[j];
+      items_total += (unsigned)(h_pl[j].wblocks * h_pl[j].hblocks + 31) / 32;
+      h_sub_end[off + ns++] = items_total;
+    }
+    Fdct8Plane* d_pl;
+    unsigned* d_pl_end;
+    if ((rc = upload_plan(ws_, h_sub + off, ns, &d_pl)) || (rc = upload_plan(ws_, h_sub_end + off, ns, &d_pl_end))) return rc;
+    TIMED(ws_, "fdct_code_batch", launch_fdct8_code_batch(d_pl, d_pl_end, (unsigned)ns, items_total, q[pi], ws_.stream()));
+    off += ns;
+  }
   if ((rc = jpeg_entropy_batch_dev(ws_, enc, nenc))) return rc;
   // 6. two host waits: every scan's size, then every scan's bytes
   if ((rc = ws_.sync())) return rc;
@@ -421,7 +457,7 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
     if (it.rc) continue;
     int r = jpeg_scan_check(it.base_jpeg);   // in transcode()'s order
     if (!r) r = jpeg_scan_check(it.gm_jpeg);
-    if (!r) r = transcode_finish(it.data, it.info, it.ph, it.gh, it.base_jpeg, it.gm_jpeg, cfg, it.out, it.cap, &it.out_size);
+    if (!r) r = transcode_finish(it.data, it.info, it.ph, it.gh, it.base_jpeg, it.gm_jpeg, it.cfg, it.out, it.cap, &it.out_size);
     if (r) batch_fail(it, r, last_error());
   }
   return E_OK;

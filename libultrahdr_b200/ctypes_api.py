@@ -183,6 +183,18 @@ def declare_transcode_batch(lib):
     return lib
 
 
+class TranscodeRung(C.Structure):
+    """uhdr_b200_transcode_rung_t: one output of uhdr_b200_transcode_ladder"""
+    _fields_ = [("cfg", TranscodeConfig), ("out", C.c_void_p), ("cap", C.c_size_t), ("out_size", C.c_size_t),
+                ("status", C.c_int)]
+
+
+def declare_transcode_ladder(lib):
+    """argument types of uhdr_b200_transcode_ladder (include/uhdr_b200.h) on a loaded libuhdr_b200"""
+    lib.uhdr_b200_transcode_ladder.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(TranscodeRung), C.c_int]
+    return lib
+
+
 def jpeg_encode_batch_stats(lib):
     """-> (k_huff_encode_batch launches, scans they coded) since process start"""
     st = (C.c_ulonglong * 2)()
