@@ -416,6 +416,8 @@ UHDR_API uhdr_error_info_t uhdr_encode(uhdr_codec_private_t* enc) {
     else
       rc = h->codec.encode(*hdr_in, sdr_in, cfg, h->quality[UHDR_BASE_IMG],
                            h->exif.empty() ? nullptr : h->exif.data(), h->exif.size(), h->out.get(), cap, &n);
+    // a failed call can leave copies from the pinned arena in flight, and the next one rewinds it
+    if (rc) cudaStreamSynchronize(h->codec.ws().stream());
   }
   h->status = from_rc(rc);
   if (rc == E_OK) {
@@ -644,7 +646,10 @@ static JpegRCodec* tls_codec() {
     c = new JpegRCodec();
     if (c->init() != E_OK) { delete c; c = nullptr; }
   }
-  if (c) c->ws().rewind();
+  if (c) {  // an earlier call that failed can have left copies from the pinned arena in flight
+    c->ws().sync();
+    c->ws().rewind();
+  }
   return c;
 }
 

@@ -465,30 +465,36 @@ int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, 
   return E_OK;
 }
 
+// the inverse DCT of a decode planned by decode_jpeg_plan, its coefficients on the device
+static JpegIdctJob idct_job(const JpegHeader& h, const JpegDecodeJob& j, int16_t* const d_coefs[3]) {
+  JpegIdctJob o;
+  o.h = &h;
+  o.g = j.k != 1 ? &j.g : nullptr;
+  for (int c = 0; c < 3; c++) {
+    o.d_coefs[c] = d_coefs[c];
+    o.planes[c] = j.planes[c];
+    o.strides[c] = j.strides[c];
+  }
+  return o;
+}
+
 int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size, int mode, DevImage* out, JpegHeader* h,
                                 YccToRgbaParams* to_rgba, int k) {
   JpegDecodeJob j;
   int rc = decode_jpeg_begin(ws, data, size, mode, k, out, h, &j);
   if (rc) return rc;
   const JpegFrame& f = h->frame;
-  const bool scaled = k != 1;
-  const JpegScaled& g = j.g;
-  uint8_t** planes = j.planes;
-  int* strides = j.strides;
   // entropy decoding: on the device (huffdec.cu).  The host decoder is not a size-based alternative: it runs only
   // for streams the parallel decoder declines (restart markers, no fixed point, inconsistent data -- it also
   // produces the reference's error texts for those) or when a test / triage session selects it (mode 1).
-  const int dec_mode = jpeg_get_entropy_decoder();
-  bool on_device = dec_mode != 1;
+  int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
+  bool on_device = jpeg_get_entropy_decoder() != 1;
   if (on_device) {
-    int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
     rc = jpeg_entropy_decode_dev(ws, data, size, *h, d_coefs);
     if (rc == kHuffDecFallback) on_device = false;
     else if (rc) return rc;
-    else rc = scaled ? jpeg_idct_scaled_dev(ws, *h, g, d_coefs, planes, strides) : jpeg_idct_dev(ws, *h, d_coefs, planes, strides);
-    if (on_device && rc) return rc;
   }
-  if (!on_device) {
+  if (!on_device) {  // the host decoder's coefficients, then their copy to the device
     int16_t* h_coefs[3] = {nullptr, nullptr, nullptr};
     for (int c = 0; c < f.ncomp; c++) {
       h_coefs[c] = (int16_t*)ws.halloc(f.blocks(c) * 128);
@@ -496,9 +502,14 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
     }
     rc = jpeg_host_decode_coefs(data, size, *h, h_coefs);
     if (rc) return rc;
-    rc = scaled ? jpeg_inverse_scaled_dev(ws, *h, g, h_coefs, planes, strides) : jpeg_inverse_dev(ws, *h, h_coefs, planes, strides);
-    if (rc) return rc;
+    for (int c = 0; c < f.ncomp; c++) {
+      d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
+      if (!d_coefs[c]) return E_MEM;
+      CUDA_TRY(cudaMemcpyAsync(d_coefs[c], h_coefs[c], f.blocks(c) * 128, cudaMemcpyHostToDevice, ws.stream()));
+    }
   }
+  const JpegIdctJob job = idct_job(*h, j, d_coefs);
+  if ((rc = jpeg_idct_dev(ws, &job, 1))) return rc;
   return decode_jpeg_end(ws, h, j, out, to_rgba);
 }
 
@@ -848,16 +859,6 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
   // these modes), the map header's error, the map's result; then one inverse DCT for everything that is left
   JpegIdctJob* jobs = batch_idct_.data();
   int nj = 0, si = 0;
-  auto add_job = [&](const JpegHeader& h, const JpegDecodeJob& j, const JpegBatchScan& sc) {
-    JpegIdctJob& o = jobs[nj++];
-    o.h = &h;
-    o.g = j.k != 1 ? &j.g : nullptr;
-    for (int c = 0; c < 3; c++) {
-      o.d_coefs[c] = sc.d_coefs[c];
-      o.planes[c] = j.planes[c];
-      o.strides[c] = j.strides[c];
-    }
-  };
   for (int i = 0; i < n; i++) {
     BatchFile& f = items[i];
     if (f.rc) continue;
@@ -880,10 +881,10 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
       batch_fail(f, gs->rc, gs->err);
       continue;
     }
-    add_job(f.ph, f.pj, ps);
-    if (gs) add_job(f.gh, f.gj, *gs);
+    jobs[nj++] = idct_job(f.ph, f.pj, ps.d_coefs);
+    if (gs) jobs[nj++] = idct_job(f.gh, f.gj, gs->d_coefs);
   }
-  if (nj && (rc = jpeg_idct_batch_dev(ws_, jobs, nj))) return rc;
+  if (nj && (rc = jpeg_idct_dev(ws_, jobs, nj))) return rc;
   // 4. per file, the map's tail stage -- after the inverse DCT: a 3-channel map in mode 2 launches its colour conversion
   // there -- and the gamuts of both ICC profiles
   for (int i = 0; i < n; i++) {
@@ -962,7 +963,7 @@ int JpegRCodec::decode_ladder(const uint8_t* data, const DecodedInfo& info, Tran
   const JpegBatchScan* ps = &scans[0];
   const JpegBatchScan* gs = need_g ? &scans[1] : nullptr;
   // 3. per k in transcode()'s order: the primary's scan and tail stage, the map's plan, scan and tail stage (mode 0
-  // launches nothing there); then one k_idct_multi over both JPEGs at every k left
+  // launches nothing there); then one k_idct<0> over both JPEGs at every k left
   auto fail_k = [](LadderK& K, int r, const char* msg) {
     K.rc = r;
     snprintf(K.err, sizeof K.err, "%s", msg);
@@ -985,32 +986,22 @@ int JpegRCodec::decode_ladder(const uint8_t* data, const DecodedInfo& info, Tran
       fail_k(K, r, last_error());
     }
   }
-  IdctMultiPlane* pl = (IdctMultiPlane*)ws_.halloc(sizeof(IdctMultiPlane) * 6);
+  IdctPlane* pl = jpeg_idct_stage(ws_, 6);
   if (!pl) return E_MEM;
   int np = 0;
   for (int m = 0; m < 2; m++) {
-    const JpegHeader& h = m ? gh : ph;
-    const JpegFrame& f = h.frame;
+    const JpegFrame& f = (m ? gh : ph).frame;
+    const JpegBatchScan* sc = m ? gs : ps;   // read only for a k that is left, whose scans were decoded
     for (int c = 0; c < f.ncomp; c++) {
-      IdctMultiPlane& P = pl[np];
-      memset(&P, 0, sizeof P);
-      const JpegComp& comp = f.comp[c];
-      memcpy(P.q, f.qt[comp.tq], sizeof P.q);
-      P.wblocks = comp.wblocks;
-      P.blocks = comp.wblocks * comp.hblocks;
+      IdctPlane& P = pl[np];
+      P.nout = 0;
       for (int j = 0; j < nk; j++) {
         const LadderK& K = ks[j];
         if (K.rc) continue;
         const JpegDecodeJob& job = m ? K.gj : K.pj;
-        IdctMultiPlane::Out& o = P.out[P.nout++];
-        o.s = K.k == 1 ? 8 : job.g.s[c];
-        o.dst = job.planes[c];
-        o.dst_stride = job.strides[c];
-        o.dst_w = o.s == 8 ? std::min(comp.wblocks * 8, o.dst_stride) : comp.wblocks * o.s;
-        o.dst_h = comp.hblocks * o.s;
+        jpeg_idct_plane(&P, f, c, sc->d_coefs[c], K.k == 1 ? 8 : job.g.s[c], job.planes[c], job.strides[c]);
       }
       if (!P.nout) break;   // no k is left
-      P.coefs = (m ? gs : ps)->d_coefs[c];
       np++;
     }
   }

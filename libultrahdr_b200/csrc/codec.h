@@ -150,7 +150,7 @@ class JpegRCodec {
   int decode_images(const uint8_t* data, size_t size, const DecodedInfo& probed, int k, DevImage* sdr, DevImage* map,
                     uhdr_gainmap_metadata_t* md);
   // decode() into device planes (dev_stream, k) of many files, with one entropy decoding and one inverse DCT for all of
-  // them (jpeg_entropy_decode_batch_dev, jpeg_idct_batch_dev), then each file's colour conversion / gain-map
+  // them (jpeg_entropy_decode_batch_dev, jpeg_idct_dev), then each file's colour conversion / gain-map
   // application into its planes.  Each item gets the bytes and the code decode() gives for it alone; a failing item
   // writes nothing.  Items are taken in groups that fit `group_bytes` of scratch.  The writes are ordered after the
   // work enqueued earlier on `caller`, which waits for them; settle() waits for them on the host.  The return value is
@@ -184,7 +184,7 @@ class JpegRCodec {
   // failing item writes nothing.  The return value is an error that ends the whole call (CUDA, memory).
   int transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg, size_t group_bytes);
   // transcode() of one file (`data`, `info` its probe()) into n <= kLadderMaxRungs outputs, each with its own cfg: both
-  // JPEGs entropy-decoded once, one k_idct_multi launch for every k the rungs ask for, then the batch's encode
+  // JPEGs entropy-decoded once, one k_idct<0> launch for every k the rungs ask for, then the batch's encode
   // (transcode_encode).  rungs[i].rc != E_OK on entry skips the rung.  Each rung gets the bytes, size and code
   // transcode() gives for its cfg alone; a failing rung writes nothing.  The return value is an error that ends the
   // whole call (CUDA, memory).
@@ -228,7 +228,7 @@ class JpegRCodec {
   int decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller);
   int transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg);
   // transcode_ladder's decode: the headers once, per distinct k the plans of both JPEGs, one entropy decoding of each
-  // scan, the errors in transcode()'s order per k, one k_idct_multi; then each rung's decoded pair (sdr, map, ph, gh)
+  // scan, the errors in transcode()'s order per k, one k_idct<0>; then each rung's decoded pair (sdr, map, ph, gh)
   int decode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n);
   // Both transcode paths' encode, once every item's pair is decoded: per item its cfg's 4:2:2 check of base_420, one
   // k_stage_batch launch, one k_fdct8_code_batch launch per distinct (base_quality, gainmap_quality) pair (at most

@@ -56,6 +56,7 @@ JpegRCodec* tls_codec(int* rc) {
       return nullptr;
     }
   }
+  c->ws().sync();  // an earlier call that failed can have left copies from the pinned arena in flight
   c->ws().rewind();
   return c;
 }

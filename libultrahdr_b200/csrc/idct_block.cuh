@@ -1,8 +1,7 @@
-// The inverse DCT of one 8x8 coefficient block, the bodies every IDCT kernel calls (k_idct_dequant and its batch form in
-// kernels.cu; k_idct_scaled, its batch form and k_idct_multi in idct_scaled.cu):
+// The inverse DCT of one 8x8 coefficient block, the bodies the IDCT kernels of idct.cu call:
 //  - idct_dequant_block: libjpeg-turbo jidctint.c "islow" (LL&M, CONST_BITS 13, PASS1_BITS 2), dequantised with the
 //    raw quantiser values, +128 and a saturating clamp (the semantics of the SIMD forms the library runs);
-//  - idct_scaled_block<S>, S = 4 / 2 / 1: jidctred.c (jpeg_idct_4x4 / _2x2 / _1x1), described in idct_scaled.cu.
+//  - idct_scaled_block<S>, S = 4 / 2 / 1: jidctred.c (jpeg_idct_4x4 / _2x2 / _1x1), described in idct.cu.
 // Integer arithmetic, bit-exact.
 #pragma once
 #include <cstdint>

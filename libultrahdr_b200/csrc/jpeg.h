@@ -124,11 +124,6 @@ struct JpegHeader {
 int jpeg_read_header(const uint8_t* data, size_t size, JpegHeader* h);
 // entropy-decode into [block][64] natural-order coefficient arrays (host)
 int jpeg_host_decode_coefs(const uint8_t* data, size_t size, const JpegHeader& h, int16_t* coefs[3]);
-// Enqueue H2D of coefficients + dequant/IDCT into device planes (stride = wblocks*8).
-int jpeg_inverse_dev(Workspace& ws, const JpegHeader& h, int16_t* const h_coefs[3],
-                     uint8_t* d_planes[3], int plane_stride[3]);
-// Same, coefficients already on the device.
-int jpeg_idct_dev(Workspace& ws, const JpegHeader& h, int16_t* const d_coefs[3], uint8_t* d_planes[3], int plane_stride[3]);
 // Reduced-size decoding, libjpeg's scale_num = 1, scale_denom = k (jdmaster.c): the output is ceil(W/k) x ceil(H/k).
 // Every component starts at a DCT scaled size of 8/k samples per block side, doubled while that is < 8 and the
 // sampling factors allow it (chroma is scaled up by the IDCT, not by an upsampler): a 4:2:0 frame comes out 4:4:4.
@@ -140,11 +135,14 @@ struct JpegScaled {
 };
 // E_INVALID_PARAM for k outside {1, 2, 4, 8}
 int jpeg_scaled_geometry(const JpegFrame& f, int k, JpegScaled* g);
-// Dequant + IDCT at the scaled sizes: components of size 8 through k_idct_dequant, the others through the reduced
-// IDCT (one launch per size).  Plane c holds hblocks*s[c] rows of wblocks*s[c] samples at plane_stride[c].
-int jpeg_idct_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const d_coefs[3],
-                         uint8_t* d_planes[3], int plane_stride[3]);
-// One JPEG of a batched inverse DCT: g null for the full size (jpeg_idct_dev), else jpeg_idct_scaled_dev's geometry
+// Dequant + IDCT (idct.cu).  Component c of a decode comes out at DCT scaled size s (8 at full size, JpegScaled::s[c]
+// at 1/k): hblocks*s rows of wblocks*s samples at its plane's stride, clipped to the stride at s = 8.
+// Pinned room in the workspace's arena for n planes of an IDCT launch and their CTA ends
+IdctPlane* jpeg_idct_stage(Workspace& ws, int n);
+// Adds to p the output of component c of frame f at size s into dst at `stride`; the plane's first output (p->nout = 0)
+// also sets its coefficients (device, [block][64] natural order), quantiser and block counts
+void jpeg_idct_plane(IdctPlane* p, const JpegFrame& f, int c, const int16_t* coefs, int s, uint8_t* dst, int stride);
+// One JPEG of an inverse DCT: g null for the full size, else the geometry of its 1/k decode
 struct JpegIdctJob {
   const JpegHeader* h;
   const JpegScaled* g;
@@ -152,14 +150,12 @@ struct JpegIdctJob {
   uint8_t* planes[3];
   int strides[3];
 };
-// The bytes jpeg_idct_dev / jpeg_idct_scaled_dev write for each job, with one launch per DCT scaled size for all of them
-int jpeg_idct_batch_dev(Workspace& ws, const JpegIdctJob* jobs, int n);
-// One launch of k_idct_multi over `planes` (host memory, n entries, copied to the device on ws.stream()): each plane's
-// coefficients are read once and written at every size its outputs ask for
-int jpeg_idct_multi_dev(Workspace& ws, const IdctMultiPlane* planes, int n);
-// Same, coefficients decoded on the host.
-int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const h_coefs[3],
-                            uint8_t* d_planes[3], int plane_stride[3]);
+// Every plane of every job, enqueued on ws.stream(): one copy of the planes to the device, then one k_idct<s> launch per
+// size s for all of them
+int jpeg_idct_dev(Workspace& ws, const JpegIdctJob* jobs, int n);
+// One k_idct<0> launch over planes[0, n) of a jpeg_idct_stage, after one copy to the device: each plane's coefficients
+// are read once and written at every size its outputs ask for
+int jpeg_idct_multi_dev(Workspace& ws, IdctPlane* planes, int n);
 // Entropy decoding on the device (huffdec.cu): fills d_coefs[c] (allocated from the workspace) with
 // [block][64] natural-order coefficients.  Returns kHuffDecFallback when the stream is outside what
 // the parallel decoder handles (restart markers, no fixed point, inconsistent data): the caller then

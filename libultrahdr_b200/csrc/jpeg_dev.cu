@@ -1,4 +1,5 @@
 // Device orchestration of the JPEG block stage (see jpeg.h).
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstring>
@@ -102,141 +103,87 @@ int jpeg_forward_plan(Workspace& ws, const DevImage& img, int quality, JpegEncod
   return E_OK;
 }
 
-int jpeg_idct_dev(Workspace& ws, const JpegHeader& h, int16_t* const d_coefs[3], uint8_t* d_planes[3], int plane_stride[3]) {
-  const JpegFrame& f = h.frame;
-  for (int c = 0; c < f.ncomp; c++) {
-    const JpegComp& k = f.comp[c];
-    IdctPlaneParams p;
-    memset(&p, 0, sizeof p);
-    p.coefs = d_coefs[c];
-    memcpy(p.q, f.qt[k.tq], sizeof p.q);
-    p.wblocks = k.wblocks;
-    p.hblocks = k.hblocks;
-    p.dst = d_planes[c];
-    p.dst_stride = plane_stride[c];
-    p.dst_w = k.wblocks * 8 < plane_stride[c] ? k.wblocks * 8 : plane_stride[c];
-    p.dst_h = k.hblocks * 8;
-    TIMED(ws, "idct_dequant", launch_idct_dequant(p, ws.stream()));
+IdctPlane* jpeg_idct_stage(Workspace& ws, int n) {
+  return (IdctPlane*)ws.halloc((sizeof(IdctPlane) + sizeof(unsigned)) * n);
+}
+
+void jpeg_idct_plane(IdctPlane* p, const JpegFrame& f, int c, const int16_t* coefs, int s, uint8_t* dst, int stride) {
+  const JpegComp& k = f.comp[c];
+  if (!p->nout) {
+    p->coefs = coefs;
+    memcpy(p->q, f.qt[k.tq], sizeof p->q);
+    p->wblocks = k.wblocks;
+    p->blocks = k.wblocks * k.hblocks;
   }
+  IdctPlane::Out& o = p->out[p->nout++];
+  o.dst = dst;
+  o.s = s;
+  o.dst_stride = stride;
+  o.dst_w = s == 8 ? std::min(k.wblocks * 8, stride) : k.wblocks * s;
+  o.dst_h = k.hblocks * s;
+}
+
+namespace {
+// planes[0, n) of a jpeg_idct_stage and the CTA ends after them, end[n] (each run of planes launched together counts
+// from 0), to the device with one copy
+int idct_upload(Workspace& ws, const IdctPlane* planes, int n, IdctPlane** d_pl, unsigned** d_end) {
+  const size_t bytes = (sizeof(IdctPlane) + sizeof(unsigned)) * n;
+  *d_pl = (IdctPlane*)ws.dalloc(bytes);
+  if (!*d_pl) return E_MEM;
+  *d_end = (unsigned*)(*d_pl + n);
+  CUDA_TRY(cudaMemcpyAsync(*d_pl, planes, bytes, cudaMemcpyHostToDevice, ws.stream()));
   return E_OK;
 }
+}  // namespace
 
-int jpeg_inverse_dev(Workspace& ws, const JpegHeader& h, int16_t* const h_coefs[3], uint8_t* d_planes[3],
-                     int plane_stride[3]) {
-  const JpegFrame& f = h.frame;
-  int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
-  for (int c = 0; c < f.ncomp; c++) {
-    d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
-    if (!d_coefs[c]) return E_MEM;
-    CUDA_TRY(cudaMemcpyAsync(d_coefs[c], h_coefs[c], f.blocks(c) * 128, cudaMemcpyHostToDevice, ws.stream()));
-  }
-  return jpeg_idct_dev(ws, h, d_coefs, d_planes, plane_stride);
-}
-
-int jpeg_idct_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const d_coefs[3],
-                         uint8_t* d_planes[3], int plane_stride[3]) {
-  const JpegFrame& f = h.frame;
-  for (int c = 0; c < f.ncomp; c++) {
-    if (g.s[c] != 8) continue;
-    const JpegComp& k = f.comp[c];
-    IdctPlaneParams p;
-    memset(&p, 0, sizeof p);
-    p.coefs = d_coefs[c];
-    memcpy(p.q, f.qt[k.tq], sizeof p.q);
-    p.wblocks = k.wblocks;
-    p.hblocks = k.hblocks;
-    p.dst = d_planes[c];
-    p.dst_stride = plane_stride[c];
-    p.dst_w = k.wblocks * 8 < plane_stride[c] ? k.wblocks * 8 : plane_stride[c];
-    p.dst_h = k.hblocks * 8;
-    TIMED(ws, "idct_dequant", launch_idct_dequant(p, ws.stream()));
-  }
-  for (int size = 4; size >= 1; size /= 2) {
-    IdctScaledParams p;
-    memset(&p, 0, sizeof p);
-    int blocks = 0;
-    for (int c = 0; c < f.ncomp; c++) {
-      if (g.s[c] != size) continue;
-      const JpegComp& k = f.comp[c];
-      IdctScaledParams::Plane& pl = p.plane[p.nplanes];
-      pl.coefs = d_coefs[c];
-      memcpy(pl.q, f.qt[k.tq], sizeof pl.q);
-      pl.wblocks = k.wblocks;
-      pl.dst = d_planes[c];
-      pl.dst_stride = plane_stride[c];
-      pl.dst_w = k.wblocks * size;
-      pl.dst_h = k.hblocks * size;
-      blocks += k.wblocks * k.hblocks;
-      p.block_end[p.nplanes++] = blocks;
-    }
-    if (p.nplanes) TIMED(ws, "idct_scaled", launch_idct_scaled(p, size, ws.stream()));
-  }
-  return E_OK;
-}
-
-int jpeg_inverse_scaled_dev(Workspace& ws, const JpegHeader& h, const JpegScaled& g, int16_t* const h_coefs[3],
-                            uint8_t* d_planes[3], int plane_stride[3]) {
-  const JpegFrame& f = h.frame;
-  int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
-  for (int c = 0; c < f.ncomp; c++) {
-    d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
-    if (!d_coefs[c]) return E_MEM;
-    CUDA_TRY(cudaMemcpyAsync(d_coefs[c], h_coefs[c], f.blocks(c) * 128, cudaMemcpyHostToDevice, ws.stream()));
-  }
-  return jpeg_idct_scaled_dev(ws, h, g, d_coefs, d_planes, plane_stride);
-}
-
-int jpeg_idct_batch_dev(Workspace& ws, const JpegIdctJob* jobs, int n) {
-  const size_t cap = 3 * (size_t)n;
-  for (int size = 8; size >= 1; size /= 2) {
-    IdctBatchPlane* h_pl = (IdctBatchPlane*)ws.halloc(sizeof(IdctBatchPlane) * cap);
-    unsigned* h_end = (unsigned*)ws.halloc(sizeof(unsigned) * cap);
-    if (!h_pl || !h_end) return E_MEM;
-    unsigned np = 0, ctas = 0;
+int jpeg_idct_dev(Workspace& ws, const JpegIdctJob* jobs, int n) {
+  int np = 0;
+  for (int i = 0; i < n; i++) np += jobs[i].h->frame.ncomp;
+  IdctPlane* h_pl = jpeg_idct_stage(ws, np);
+  if (!h_pl) return E_MEM;
+  unsigned* h_end = (unsigned*)(h_pl + np);
+  // the planes by size, 8 first: run r (size 8 >> r) is planes [first[r], first[r + 1]), ctas[r] CTAs
+  int first[5], m = 0;
+  unsigned ctas[4];
+  for (int r = 0; r < 4; r++) {
+    first[r] = m;
+    ctas[r] = 0;
     for (int i = 0; i < n; i++) {
       const JpegFrame& f = jobs[i].h->frame;
       for (int c = 0; c < f.ncomp; c++) {
-        if ((jobs[i].g ? jobs[i].g->s[c] : 8) != size) continue;
-        const JpegComp& k = f.comp[c];
-        IdctBatchPlane& p = h_pl[np];
-        p.coefs = jobs[i].d_coefs[c];
-        memcpy(p.q, f.qt[k.tq], sizeof p.q);
-        p.wblocks = k.wblocks;
-        p.blocks = k.wblocks * k.hblocks;
-        p.dst = jobs[i].planes[c];
-        p.dst_stride = jobs[i].strides[c];
-        p.dst_w = size == 8 ? (k.wblocks * 8 < p.dst_stride ? k.wblocks * 8 : p.dst_stride) : k.wblocks * size;
-        p.dst_h = k.hblocks * size;
-        ctas += (unsigned)(p.blocks + 127) / 128;
-        h_end[np++] = ctas;
+        const int s = jobs[i].g ? jobs[i].g->s[c] : 8;
+        if (s != 8 >> r) continue;
+        IdctPlane& p = h_pl[m];
+        p.nout = 0;
+        jpeg_idct_plane(&p, f, c, jobs[i].d_coefs[c], s, jobs[i].planes[c], jobs[i].strides[c]);
+        ctas[r] += (unsigned)(p.blocks + 127) / 128;
+        h_end[m++] = ctas[r];
       }
     }
-    if (!np) continue;
-    IdctBatchPlane* d_pl = (IdctBatchPlane*)ws.dalloc(sizeof(IdctBatchPlane) * np);
-    unsigned* d_end = (unsigned*)ws.dalloc(sizeof(unsigned) * np);
-    if (!d_pl || !d_end) return E_MEM;
-    CUDA_TRY(cudaMemcpyAsync(d_pl, h_pl, sizeof(IdctBatchPlane) * np, cudaMemcpyHostToDevice, ws.stream()));
-    CUDA_TRY(cudaMemcpyAsync(d_end, h_end, sizeof(unsigned) * np, cudaMemcpyHostToDevice, ws.stream()));
-    if (size == 8) TIMED(ws, "idct_dequant_batch", launch_idct_dequant_batch(d_pl, d_end, np, ctas, ws.stream()));
-    else TIMED(ws, "idct_scaled_batch", launch_idct_scaled_batch(d_pl, d_end, np, ctas, size, ws.stream()));
+  }
+  first[4] = m;
+  IdctPlane* d_pl;
+  unsigned* d_end;
+  if (int rc = idct_upload(ws, h_pl, np, &d_pl, &d_end)) return rc;
+  for (int r = 0; r < 4; r++) {
+    const unsigned k = (unsigned)(first[r + 1] - first[r]);
+    if (k)
+      TIMED(ws, r ? "idct_scaled" : "idct_dequant", launch_idct(8 >> r, d_pl + first[r], d_end + first[r], k, ctas[r], ws.stream()));
   }
   return E_OK;
 }
 
-int jpeg_idct_multi_dev(Workspace& ws, const IdctMultiPlane* planes, int n) {
-  unsigned* h_end = (unsigned*)ws.halloc(sizeof(unsigned) * n);
-  if (!h_end) return E_MEM;
+int jpeg_idct_multi_dev(Workspace& ws, IdctPlane* planes, int n) {
+  unsigned* h_end = (unsigned*)(planes + n);
   unsigned ctas = 0;
   for (int i = 0; i < n; i++) {
     ctas += (unsigned)(planes[i].blocks + 127) / 128;
     h_end[i] = ctas;
   }
-  IdctMultiPlane* d_pl = (IdctMultiPlane*)ws.dalloc(sizeof(IdctMultiPlane) * n);
-  unsigned* d_end = (unsigned*)ws.dalloc(sizeof(unsigned) * n);
-  if (!d_pl || !d_end) return E_MEM;
-  CUDA_TRY(cudaMemcpyAsync(d_pl, planes, sizeof(IdctMultiPlane) * n, cudaMemcpyHostToDevice, ws.stream()));
-  CUDA_TRY(cudaMemcpyAsync(d_end, h_end, sizeof(unsigned) * n, cudaMemcpyHostToDevice, ws.stream()));
-  TIMED(ws, "idct_multi", launch_idct_multi(d_pl, d_end, (unsigned)n, ctas, ws.stream()));
+  IdctPlane* d_pl;
+  unsigned* d_end;
+  if (int rc = idct_upload(ws, planes, n, &d_pl, &d_end)) return rc;
+  TIMED(ws, "idct_multi", launch_idct(0, d_pl, d_end, (unsigned)n, ctas, ws.stream()));
   return E_OK;
 }
 

@@ -7,7 +7,6 @@
 
 #include <atomic>
 
-#include "idct_block.cuh"
 #include "powf_glibc.cuh"
 #include "tables.h"
 
@@ -716,36 +715,9 @@ __global__ void __launch_bounds__(256) k_yuv_convert(const YuvConvParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// JPEG block stage: libjpeg-turbo jfdctint.c / jidctint.c "islow" (LL&M, CONST_BITS 13,
-// PASS1_BITS 2), jcdctmgr.c quantiser (divisor 8*Q, round half away from zero), jccolor.c /
-// jdcolor.c colour conversion.  Integer arithmetic, bit-exact.
+// JPEG decoder colour stage: jdcolor.c colour conversion, integer arithmetic, bit-exact (the forward block stage lives in
+// fdct8.cu, the inverse DCT in idct.cu).
 // ------------------------------------------------------------------------------------------------
-
-// (the forward block stage lives in fdct8.cu, the inverse DCT's block bodies in idct_block.cuh)
-
-__global__ void __launch_bounds__(128) k_idct_dequant(const IdctPlaneParams p) {
-  const int bx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int by = blockIdx.y;
-  __shared__ uint16_t sq[64];
-  if (threadIdx.x < 64) sq[threadIdx.x] = p.q[threadIdx.x];
-  __syncthreads();
-  if (bx >= p.wblocks) return;
-  idct_dequant_block(p.coefs, sq, p.wblocks, bx, by, p.dst, p.dst_stride, p.dst_w, p.dst_h);
-}
-
-// every plane of a batch in one launch: each CTA covers 128 blocks of one plane
-__global__ void __launch_bounds__(128) k_idct_dequant_batch(const IdctBatchPlane* __restrict__ planes, const unsigned* __restrict__ cta_end,
-                                                            unsigned n) {
-  const unsigned j = batch_find(cta_end, n, blockIdx.x);
-  const IdctBatchPlane& p = planes[j];
-  __shared__ uint16_t sq[64];
-  if (threadIdx.x < 64) sq[threadIdx.x] = p.q[threadIdx.x];
-  __syncthreads();
-  const int local = (int)(blockIdx.x - (j ? cta_end[j - 1] : 0)) * 128 + threadIdx.x;
-  if (local >= p.blocks) return;
-  const int by = local / p.wblocks, bx = local - by * p.wblocks;
-  idct_dequant_block(p.coefs, sq, p.wblocks, bx, by, p.dst, p.dst_stride, p.dst_w, p.dst_h);
-}
 
 // jdcolor.c ycc_rgb_convert with JCS_EXT_RGBA (alpha 0xFF).  ORG: a region with an origin other than 0, 0
 template <bool ORG>
@@ -930,19 +902,6 @@ cudaError_t launch_yuv_convert(const YuvConvParams& p, cudaStream_t s) {
   dim3 b(32, 8);
   const int f = p.fmt == F_YUV420 ? 2 : 1;
   k_yuv_convert<<<grid2(p.w / f, p.h / f, b), b, 0, s>>>(p);
-  COUNT_LAUNCH();
-  return cudaGetLastError();
-}
-cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s) {
-  dim3 b(128, 1);
-  dim3 g((p.wblocks + 127) / 128, p.hblocks);
-  k_idct_dequant<<<g, b, 0, s>>>(p);
-  COUNT_LAUNCH();
-  return cudaGetLastError();
-}
-cudaError_t launch_idct_dequant_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s) {
-  if (!ctas) return cudaSuccess;
-  k_idct_dequant_batch<<<ctas, 128, 0, s>>>(planes, cta_end, n);
   COUNT_LAUNCH();
   return cudaGetLastError();
 }

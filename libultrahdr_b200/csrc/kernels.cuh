@@ -147,41 +147,9 @@ struct Fdct8Params {
   const uint32_t* acbooks;          // zigzag launches: device pointer, AC code books (code << 8 | length), [0..255] luminance [256..511] chrominance (filled by launch_fdct8)
 };
 
-struct IdctPlaneParams {
-  const int16_t* coefs;
-  uint16_t q[64];
-  int wblocks, hblocks;
-  uint8_t* dst;
-  int dst_stride;                   // >= wblocks*8 unless clipped by dst_w/dst_h
-  int dst_w, dst_h;                 // samples beyond are not written
-};
-
-// reduced-size IDCT (idct_scaled.cu): the planes of one JPEG whose DCT scaled size is the launch's (4, 2 or 1)
-struct IdctScaledParams {
-  int nplanes;
-  int block_end[3];                 // cumulative block counts: plane i holds blocks [block_end[i-1], block_end[i])
-  struct Plane {
-    const int16_t* coefs;
-    uint16_t q[64];
-    int wblocks;
-    uint8_t* dst;
-    int dst_stride;                 // >= wblocks * size
-    int dst_w, dst_h;               // samples beyond are not written
-  } plane[3];
-};
-
-// one plane of a batched inverse DCT (jpeg_idct_batch_dev): many JPEGs' planes of one DCT scaled size in one launch
-struct IdctBatchPlane {
-  const int16_t* coefs;
-  uint16_t q[64];
-  int wblocks, blocks;
-  uint8_t* dst;
-  int dst_stride;
-  int dst_w, dst_h;                 // samples beyond are not written
-};
-// one plane of k_idct_multi: its coefficients decoded once, written at up to four DCT scaled sizes (the sizes a ladder of
-// 1/k decodes needs); out[i] gets the bytes k_idct_dequant (s = 8) or k_idct_scaled<s> writes for that plane
-struct IdctMultiPlane {
+// one plane of an inverse DCT launch (idct.cu): its coefficients, written at up to four DCT scaled sizes s of 8, 4, 2 or 1
+// samples per block side (the sizes a ladder of 1/k decodes needs; every other launch has one output)
+struct IdctPlane {
   const int16_t* coefs;
   uint16_t q[64];
   int wblocks, blocks, nout;
@@ -254,15 +222,10 @@ cudaError_t launch_fdct8(const Fdct8Params& p, cudaStream_t s);
 // memory, no RGB888 plane; plane.tq[0] selects q[0..3]
 cudaError_t launch_fdct8_code_batch(const Fdct8Plane* planes, const unsigned* item_end, unsigned nplanes, unsigned total_items,
                                     const uint16_t q[4][64], cudaStream_t s);
-cudaError_t launch_idct_dequant(const IdctPlaneParams& p, cudaStream_t s);
-cudaError_t launch_idct_scaled(const IdctScaledParams& p, int size, cudaStream_t s);
 // planes / cta_end: n entries in device memory, cta_end the inclusive prefix of the planes' ceil(blocks / 128) CTAs,
-// `ctas` its last entry.  size 8: k_idct_dequant's arithmetic, 4 / 2 / 1: k_idct_scaled's.
-cudaError_t launch_idct_dequant_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s);
-cudaError_t launch_idct_scaled_batch(const IdctBatchPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, int size,
-                                     cudaStream_t s);
-// k_idct_multi: planes / cta_end as for launch_idct_dequant_batch, every output of every plane in one launch
-cudaError_t launch_idct_multi(const IdctMultiPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s);
+// `ctas` its last entry.  size 8 / 4 / 2 / 1: k_idct<size> writes out[0] of every plane, whose s is `size`; size 0:
+// k_idct<0> writes every output of every plane.
+cudaError_t launch_idct(int size, const IdctPlane* planes, const unsigned* cta_end, unsigned n, unsigned ctas, cudaStream_t s);
 cudaError_t launch_ycc_to_rgba(const YccToRgbaParams& p, cudaStream_t s);
 
 // number of kernel launches issued by this library since load (bench.py's gpu_launches)

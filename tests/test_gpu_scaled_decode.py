@@ -92,7 +92,7 @@ def test_planes_equal_libjpeg_turbo(lib, layout, w, h):
 @pytest.mark.parametrize("w,h", [(17, 33), (1000, 722), (4080, 3072)])
 @pytest.mark.parametrize("layout", ["gray", "444", "420"])
 def test_planes_host_entropy_decoder_and_restart_markers(lib, layout, w, h):
-    """the host-decoder route (jpeg_inverse_scaled_dev), forced and through a stream the device decoder declines"""
+    """the host-decoder route (host coefficients copied to the device, then jpeg_idct_dev), forced and through a stream the device decoder declines"""
     a = S.image(w, h, "smooth", seed=3)
     prev = lib.uhdr_b200_set_entropy_decoder(1)
     try:

@@ -1,6 +1,6 @@
 """uhdr_b200_transcode_ladder on the GPU, at 0 tolerance: every rung of several ladders equals uhdr_b200_transcode with
 that rung's config alone (bytes, out_size, status) for every file of the batch test's corpus, and the reference
-composition for one ladder per file; the route (two scans entropy-decoded, one k_idct_multi, one staging launch, one
+composition for one ladder per file; the route (two scans entropy-decoded, one k_idct<0>, one staging launch, one
 block-stage launch per quality pair, launch counts that do not grow with the rungs); IDCT extremes at every size;
 per-rung and file-level errors that write nothing; a scan handed back to the host decoder; interleaving with other
 calls; two threads; the heap probe."""

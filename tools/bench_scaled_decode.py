@@ -1,8 +1,8 @@
 """Reduced-size decoding: uhdr_b200_decode_scaled_dev at k = 1, 2, 4, 8 into device memory (RGBA half float), on
 bench.py's 8K input (frame 7, API-1 defaults) and on a 4080x3072 file (map scale 4, a non-integer map ratio after
 scaling).  Per k: median and best of >= 20 calls, each followed by a stream synchronise; then the block-stage kernel
-times from the library's kernel-timing report (CUDA events): k_idct_dequant ("idct_dequant") against the reduced
-IDCT ("idct_scaled"), and the colour conversion and apply kernels.  On this device-output path the report holds the
+times from the library's kernel-timing report (CUDA events): k_idct<8> ("idct_dequant") against the reduced
+IDCT k_idct<4 / 2 / 1> ("idct_scaled"), and the colour conversion and apply kernels.  On this device-output path the report holds the
 gain-map JPEG's kernels, which run on the codec's second stream; the primary JPEG's are not collected.  The card's name and power limit are read
 in the same run.  Prints one JSON line.
 

@@ -6,7 +6,7 @@ Files: bench.py's 8K API-1 file (q95, map scale 1), a 4080x3072 file with map sc
 "3 sizes" = k = 2, 4, 8 at 80 / 70; base_420 and keep_exif on in every rung.  Both arms' outputs are checked equal
 before timing.  Per arm: the median wall clock per ladder over --iters iterations after 3 warm-ups, the two arms
 alternated within each iteration, and the library's kernel launches per ladder.  Then, in a separate pass with kernel
-timing on: k_idct_multi's time per ladder against the summed k_idct_dequant / k_idct_scaled times of the loop arm.  The
+timing on: k_idct<0>'s time per ladder ("idct_multi") against the summed k_idct<S> times ("idct_dequant", "idct_scaled") of the loop arm.  The
 card's name and power limit are read in the same run.  One JSON line.
 
   python tools/bench_transcode_ladder.py [--iters 15]
