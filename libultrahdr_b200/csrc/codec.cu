@@ -483,32 +483,15 @@ int JpegRCodec::decode_jpeg_dev(Workspace& ws, const uint8_t* data, size_t size,
   JpegDecodeJob j;
   int rc = decode_jpeg_begin(ws, data, size, mode, k, out, h, &j);
   if (rc) return rc;
-  const JpegFrame& f = h->frame;
-  // entropy decoding: on the device (huffdec.cu).  The host decoder is not a size-based alternative: it runs only
-  // for streams the parallel decoder declines (restart markers, no fixed point, inconsistent data -- it also
-  // produces the reference's error texts for those) or when a test / triage session selects it (mode 1).
-  int16_t* d_coefs[3] = {nullptr, nullptr, nullptr};
-  bool on_device = jpeg_get_entropy_decoder() != 1;
-  if (on_device) {
-    rc = jpeg_entropy_decode_dev(ws, data, size, *h, d_coefs);
-    if (rc == kHuffDecFallback) on_device = false;
-    else if (rc) return rc;
+  // entropy decoding: on the device (huffdec.cu), or on the host for a stream the parallel decoder declines or while a
+  // test / triage session selects the host decoder (mode 1)
+  JpegScanJob sc{data, size, h, {}, 0, {0}};
+  if ((rc = jpeg_entropy_decode_dev(ws, &sc, 1))) return rc;
+  if (sc.rc) {
+    set_last_error(sc.err);
+    return sc.rc;
   }
-  if (!on_device) {  // the host decoder's coefficients, then their copy to the device
-    int16_t* h_coefs[3] = {nullptr, nullptr, nullptr};
-    for (int c = 0; c < f.ncomp; c++) {
-      h_coefs[c] = (int16_t*)ws.halloc(f.blocks(c) * 128);
-      if (!h_coefs[c]) return E_MEM;
-    }
-    rc = jpeg_host_decode_coefs(data, size, *h, h_coefs);
-    if (rc) return rc;
-    for (int c = 0; c < f.ncomp; c++) {
-      d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
-      if (!d_coefs[c]) return E_MEM;
-      CUDA_TRY(cudaMemcpyAsync(d_coefs[c], h_coefs[c], f.blocks(c) * 128, cudaMemcpyHostToDevice, ws.stream()));
-    }
-  }
-  const JpegIdctJob job = idct_job(*h, j, d_coefs);
+  const JpegIdctJob job = idct_job(*h, j, sc.d_coefs);
   if ((rc = jpeg_idct_dev(ws, &job, 1))) return rc;
   return decode_jpeg_end(ws, h, j, out, to_rgba);
 }
@@ -833,7 +816,7 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
   // 1. per file, the header stages of both JPEGs (decode_pair's order: primary, then map)
   if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
   if ((int)batch_idct_.size() < 2 * n) batch_idct_.resize(2 * n);
-  JpegBatchScan* scans = batch_scans_.data();
+  JpegScanJob* scans = batch_scans_.data();
   int ns = 0;
   for (int i = 0; i < n; i++) {
     BatchFile& f = items[i];
@@ -846,15 +829,15 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
       batch_fail(f, rc, last_error());
       continue;
     }
-    scans[ns++] = JpegBatchScan{f.data + in.base_off, in.base_len, &f.ph, {}, 0, {0}};
+    scans[ns++] = JpegScanJob{f.data + in.base_off, in.base_len, &f.ph, {}, 0, {0}};
     if (!f.want_map) continue;
     f.map_rc = decode_jpeg_begin(ws_, f.data + in.gainmap_off, in.gainmap_len, map_mode, k, &f.map, &f.gh, &f.gj);
     if (f.map_rc == E_MEM) return E_MEM;
     if (f.map_rc) snprintf(f.map_err, sizeof f.map_err, "%s", last_error());
-    else scans[ns++] = JpegBatchScan{f.data + in.gainmap_off, in.gainmap_len, &f.gh, {}, 0, {0}};
+    else scans[ns++] = JpegScanJob{f.data + in.gainmap_off, in.gainmap_len, &f.gh, {}, 0, {0}};
   }
   // 2. entropy decoding of every scan
-  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
+  if (ns && (rc = jpeg_entropy_decode_dev(ws_, scans, ns))) return rc;
   // 3. in the order the single call meets them: the primary's result and its tail stage (which launches nothing for
   // these modes), the map header's error, the map's result; then one inverse DCT for everything that is left
   JpegIdctJob* jobs = batch_idct_.data();
@@ -862,8 +845,8 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
   for (int i = 0; i < n; i++) {
     BatchFile& f = items[i];
     if (f.rc) continue;
-    const JpegBatchScan& ps = scans[si++];
-    const JpegBatchScan* gs = f.want_map && !f.map_rc ? &scans[si++] : nullptr;
+    const JpegScanJob& ps = scans[si++];
+    const JpegScanJob* gs = f.want_map && !f.map_rc ? &scans[si++] : nullptr;
     if (ps.rc) {
       batch_fail(f, ps.rc, ps.err);
       continue;
@@ -955,13 +938,13 @@ int JpegRCodec::decode_ladder(const uint8_t* data, const DecodedInfo& info, Tran
   }
   // 2. one entropy decoding of each scan some k needs (a scan the device decoder declines goes to the host decoder)
   if ((int)batch_scans_.size() < 2) batch_scans_.resize(2);
-  JpegBatchScan* scans = batch_scans_.data();
+  JpegScanJob* scans = batch_scans_.data();
   int ns = 0;
-  if (need_p) scans[ns++] = JpegBatchScan{pd, info.base_len, &ph, {}, 0, {0}};
-  if (need_g) scans[ns++] = JpegBatchScan{gd, info.gainmap_len, &gh, {}, 0, {0}};
-  if (ns && (rc = jpeg_entropy_decode_batch_dev(ws_, scans, ns))) return rc;
-  const JpegBatchScan* ps = &scans[0];
-  const JpegBatchScan* gs = need_g ? &scans[1] : nullptr;
+  if (need_p) scans[ns++] = JpegScanJob{pd, info.base_len, &ph, {}, 0, {0}};
+  if (need_g) scans[ns++] = JpegScanJob{gd, info.gainmap_len, &gh, {}, 0, {0}};
+  if (ns && (rc = jpeg_entropy_decode_dev(ws_, scans, ns))) return rc;
+  const JpegScanJob* ps = &scans[0];
+  const JpegScanJob* gs = need_g ? &scans[1] : nullptr;
   // 3. per k in transcode()'s order: the primary's scan and tail stage, the map's plan, scan and tail stage (mode 0
   // launches nothing there); then one k_idct<0> over both JPEGs at every k left
   auto fail_k = [](LadderK& K, int r, const char* msg) {
@@ -991,7 +974,7 @@ int JpegRCodec::decode_ladder(const uint8_t* data, const DecodedInfo& info, Tran
   int np = 0;
   for (int m = 0; m < 2; m++) {
     const JpegFrame& f = (m ? gh : ph).frame;
-    const JpegBatchScan* sc = m ? gs : ps;   // read only for a k that is left, whose scans were decoded
+    const JpegScanJob* sc = m ? gs : ps;   // read only for a k that is left, whose scans were decoded
     for (int c = 0; c < f.ncomp; c++) {
       IdctPlane& P = pl[np];
       P.nout = 0;

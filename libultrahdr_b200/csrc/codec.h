@@ -150,7 +150,7 @@ class JpegRCodec {
   int decode_images(const uint8_t* data, size_t size, const DecodedInfo& probed, int k, DevImage* sdr, DevImage* map,
                     uhdr_gainmap_metadata_t* md);
   // decode() into device planes (dev_stream, k) of many files, with one entropy decoding and one inverse DCT for all of
-  // them (jpeg_entropy_decode_batch_dev, jpeg_idct_dev), then each file's colour conversion / gain-map
+  // them (jpeg_entropy_decode_dev, jpeg_idct_dev), then each file's colour conversion / gain-map
   // application into its planes.  Each item gets the bytes and the code decode() gives for it alone; a failing item
   // writes nothing.  Items are taken in groups that fit `group_bytes` of scratch.  The writes are ordered after the
   // work enqueued earlier on `caller`, which waits for them; settle() waits for them on the host.  The return value is
@@ -265,7 +265,7 @@ class JpegRCodec {
     }
     return rc;
   }
-  std::vector<JpegBatchScan> batch_scans_;   // grow-only scratch of decode_batch and transcode_batch
+  std::vector<JpegScanJob> batch_scans_;   // grow-only scratch of decode_batch and transcode_batch
   std::vector<JpegIdctJob> batch_idct_;
   std::vector<JpegEncodeJob*> batch_enc_;
   Workspace ws_;

@@ -26,8 +26,8 @@
 //   4. DC prediction (a running sum per component over the scan order, dummy edge blocks
 //      included like jdhuff.c, restarting at every interval) is a prefix sum + scatter.
 // Streams whose restart markers are irregular (see unstuff_scan), that do not reach a fixed point
-// in kMaxRounds rounds, or whose intervals do not decode to exactly their quota of blocks return
-// kHuffDecFallback and the caller uses the host decoder of jpeg_host.cpp.
+// in kMaxRounds rounds, or whose intervals do not decode to exactly their quota of blocks go to the
+// host decoder of jpeg_host.cpp.
 #include <atomic>
 #include <climits>
 #include <cstring>
@@ -176,40 +176,6 @@ __device__ __forceinline__ void stage_shared(HdShared& S, const HdShared* __rest
   __syncthreads();
 }
 
-// one relaxation step of subsequence i of the scan whose tables are *gs; a change stores `mark` into *changed
-__device__ __forceinline__ void hd_sync_seq(HdShared& S, const unsigned i, const uint32_t* __restrict__ bits, unsigned long long* out,
-                                            unsigned long long* used, unsigned* cnt, unsigned* changed, const unsigned mark,
-                                            const HdShared* __restrict__ gs, const HdSeqs& q) {
-  const unsigned nseq = gs->f.nseq;
-  // state word: bit position | (z | c << 8) << 32; an interval's first subsequence starts at its true state
-  const unsigned long long entry = i >= nseq ? 0ull
-                                   : q.first[q.iv[i]] == i ? (unsigned long long)q.lo[i]
-                                                           : *reinterpret_cast<volatile unsigned long long*>(out + i - 1);
-  const bool todo = i < nseq && entry != used[i];  // same start as last time: same result
-  // after the second round nearly every subsequence is settled: a CTA without work leaves before it
-  // stages the 6 KB of tables, so the later rounds cost little more than their launch
-  if (!__syncthreads_or(todo ? 1 : 0)) return;
-  stage_shared(S, gs);
-  if (!todo) return;
-  unsigned p = (unsigned)entry, z = (unsigned)(entry >> 32) & 0xff, c = (unsigned)(entry >> 40);
-  const HdOut none = {};
-  const unsigned n = decode_seq<false>(S, bits, p, z, c, q.lo[i + 1], 0, 0, 0, none);
-  const unsigned long long now = (unsigned long long)p | ((unsigned long long)(z | (c << 8)) << 32);
-  used[i] = entry;
-  cnt[i] = n;
-  if (now != out[i]) {
-    *reinterpret_cast<volatile unsigned long long*>(out + i) = now;
-    *changed = mark;
-  }
-}
-
-// one relaxation round, in place (64-bit states are read and written atomically)
-__global__ void __launch_bounds__(128) k_hd_sync(const uint32_t* __restrict__ bits, unsigned long long* out, unsigned long long* used, unsigned* cnt,
-                                                 unsigned* changed, const HdShared* __restrict__ gs, const HdSeqs q) {
-  __shared__ HdShared S;
-  hd_sync_seq(S, blockIdx.x * blockDim.x + threadIdx.x, bits, out, used, cnt, changed, 1u, gs, q);
-}
-
 // start bit of subsequence i < nseq and its interval *iv
 __device__ __forceinline__ unsigned hd_seq_lo(const unsigned* __restrict__ start, const unsigned* __restrict__ first, unsigned nint,
                                               unsigned i, unsigned* iv) {
@@ -223,26 +189,90 @@ __device__ __forceinline__ unsigned hd_seq_lo(const unsigned* __restrict__ start
   return start[a] + (i - first[a]) * (unsigned)kSeqBits;
 }
 
-// expands the per-interval layout built on the host (start bit and first subsequence of each interval)
-// into the per-subsequence one
-__global__ void k_hd_layout(const unsigned* __restrict__ start, const unsigned* __restrict__ first, unsigned nint, unsigned nseq,
-                            unsigned total_bits, unsigned* lo, unsigned* iv) {
-  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0) lo[nseq] = total_bits;
-  if (i >= nseq) return;
-  lo[i] = hd_seq_lo(start, first, nint, i, iv + i);
+// A batch of scans.  Scan s owns subsequence slots [seq0, seq0 + nseq + 1) of the per-subsequence arrays, seq0 a
+// multiple of 128, so that every CTA of the relaxation and writing passes works on one scan and stages one scan's
+// tables; and intervals [iv0, iv0 + nint + 1) of the per-interval arrays.  Within its slice a scan is laid out as alone.
+struct HdScan {
+  const uint32_t* bits;
+  unsigned seq0, iv0, nint;
+  HdOut o;
+};
+struct HdBatch {
+  const HdShared* gs;     // per scan
+  const HdScan* scans;
+  const uint2* ctas;      // per CTA of a launch: {scan, first slot}
+  const unsigned* start;  // per interval: start bit (local to the scan)
+  HdSeqs q;               // lo / iv / first of every scan, values local to the scan
+};
+__device__ __forceinline__ HdSeqs hd_local(const HdBatch& B, const HdScan& sc) {
+  return HdSeqs{B.q.lo + sc.seq0, B.q.iv + sc.seq0, B.q.first + sc.iv0};
 }
 
-__global__ void k_hd_init(unsigned long long* out, unsigned long long* used, unsigned* cnt, unsigned nseq, const unsigned* __restrict__ lo) {
-  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+// expands the per-interval layout built on the host (start bit and first subsequence of each interval) into the
+// per-subsequence one, and sets the initial states; one thread per slot
+__global__ void __launch_bounds__(128) k_hd_layout(const HdBatch B, unsigned* lo, unsigned* iv, unsigned long long* out,
+                                                   unsigned long long* used, unsigned* cnt) {
+  const uint2 cta = B.ctas[blockIdx.x];
+  const HdScan& sc = B.scans[cta.x];
+  const unsigned nseq = B.gs[cta.x].f.nseq, total_bits = B.gs[cta.x].f.total_bits;
+  const unsigned i = cta.y - sc.seq0 + threadIdx.x;
+  const HdSeqs q = hd_local(B, sc);
+  const unsigned* start = B.start + sc.iv0;
+  if (i == 0) lo[sc.seq0 + nseq] = total_bits;
   if (i >= nseq) return;
-  out[i] = (unsigned long long)lo[i + 1];
-  used[i] = ~0ull;
-  cnt[i] = 0;
+  unsigned iv1;
+  lo[sc.seq0 + i] = hd_seq_lo(start, q.first, sc.nint, i, iv + sc.seq0 + i);
+  out[sc.seq0 + i] = i + 1 < nseq ? (unsigned long long)hd_seq_lo(start, q.first, sc.nint, i + 1, &iv1) : (unsigned long long)total_bits;
+  used[sc.seq0 + i] = ~0ull;
+  cnt[sc.seq0 + i] = 0;
 }
 
-// exclusive prefix sum of cnt (one CTA; nseq is at most a few hundred thousand)
-__device__ __forceinline__ void hd_prefix(const unsigned* __restrict__ cnt, unsigned* __restrict__ base, unsigned n) {
+// one relaxation round over the CTAs of the scans that still need rounds, in place (64-bit states are read and
+// written atomically); a scan's change stores round + 1 into last[scan]
+__global__ void __launch_bounds__(128) k_hd_sync(const HdBatch B, unsigned long long* out, unsigned long long* used, unsigned* cnt,
+                                                 unsigned* last, const unsigned round) {
+  __shared__ HdShared S;
+  const uint2 cta = B.ctas[blockIdx.x];
+  const HdScan& sc = B.scans[cta.x];
+  const unsigned seq0 = sc.seq0;
+  const unsigned i = cta.y - seq0 + threadIdx.x;
+  const HdShared* __restrict__ gs = B.gs + cta.x;
+  const HdSeqs q = hd_local(B, sc);
+  out += seq0;
+  used += seq0;
+  cnt += seq0;
+  const unsigned nseq = gs->f.nseq;
+  // state word: bit position | (z | c << 8) << 32; an interval's first subsequence starts at its true state
+  const unsigned long long entry = i >= nseq ? 0ull
+                                   : q.first[q.iv[i]] == i ? (unsigned long long)q.lo[i]
+                                                           : *reinterpret_cast<volatile unsigned long long*>(out + i - 1);
+  const bool todo = i < nseq && entry != used[i];  // same start as last time: same result
+  // after the second round nearly every subsequence is settled: a CTA without work leaves before it
+  // stages the 6 KB of tables, so the later rounds cost little more than their launch
+  if (!__syncthreads_or(todo ? 1 : 0)) return;
+  stage_shared(S, gs);
+  if (!todo) return;
+  unsigned p = (unsigned)entry, z = (unsigned)(entry >> 32) & 0xff, c = (unsigned)(entry >> 40);
+  const HdOut none = {};
+  const unsigned n = decode_seq<false>(S, sc.bits, p, z, c, q.lo[i + 1], 0, 0, 0, none);
+  const unsigned long long now = (unsigned long long)p | ((unsigned long long)(z | (c << 8)) << 32);
+  used[i] = entry;
+  cnt[i] = n;
+  if (now != out[i]) {
+    *reinterpret_cast<volatile unsigned long long*>(out + i) = now;
+    last[cta.x] = round + 1;
+  }
+}
+
+// exclusive prefix sum of the block counts of each scan that had rounds: one CTA per scan (nseq is at most a few
+// hundred thousand)
+__global__ void __launch_bounds__(1024) k_hd_scan(const HdBatch B, const unsigned* __restrict__ which, const unsigned* __restrict__ cnt,
+                                                  unsigned* __restrict__ base) {
+  const unsigned scan = which[blockIdx.x];
+  const unsigned seq0 = B.scans[scan].seq0;
+  const unsigned n = B.gs[scan].f.nseq;
+  cnt += seq0;
+  base += seq0;
   __shared__ unsigned warp_sums[32];
   __shared__ unsigned carry;
   if (threadIdx.x == 0) carry = 0;
@@ -273,15 +303,21 @@ __device__ __forceinline__ void hd_prefix(const unsigned* __restrict__ cnt, unsi
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(1024) k_hd_scan(const unsigned* __restrict__ cnt, unsigned* __restrict__ base, unsigned n) {
-  hd_prefix(cnt, base, n);
-}
 
-// the writing pass for subsequence i, tables staged in S.  out and base are read only for subsequences that do not
-// start an interval
-__device__ __forceinline__ void hd_write_seq(const HdShared& S, const unsigned i, const uint32_t* __restrict__ bits,
-                                             const unsigned long long* __restrict__ out, const unsigned* __restrict__ base,
-                                             const HdSeqs& q, const HdOut& o) {
+// the writing pass: each subsequence decoded once more from its entry state, tables staged in S.  out and base are read
+// only for subsequences that do not start an interval
+__global__ void __launch_bounds__(128) k_hd_write(const HdBatch B, const unsigned long long* __restrict__ out,
+                                                  const unsigned* __restrict__ base) {
+  __shared__ HdShared S;
+  const uint2 cta = B.ctas[blockIdx.x];
+  stage_shared(S, B.gs + cta.x);
+  const HdScan& sc = B.scans[cta.x];
+  const unsigned seq0 = sc.seq0;
+  const unsigned i = cta.y - seq0 + threadIdx.x;
+  const HdSeqs q = hd_local(B, sc);
+  const HdOut& o = sc.o;
+  out += seq0;
+  base += seq0;
   if (i >= S.f.nseq) return;
   const unsigned k = q.iv[i], head = q.first[k], next = q.first[k + 1];
   const unsigned long long entry = head == i ? (unsigned long long)q.lo[i] : out[i - 1];
@@ -290,82 +326,8 @@ __device__ __forceinline__ void hd_write_seq(const HdShared& S, const unsigned i
   const unsigned b = b0 + (head == i ? 0u : base[i] - base[head]);
   const unsigned b_end = min(b0 + S.f.iv_blocks, S.f.total_blocks);
   if (b % (unsigned)S.f.bpm != c) *o.err = 2;  // the states and the block counts must agree
-  const unsigned n = decode_seq<true>(S, bits, p, z, c, q.lo[i + 1], b, b_end, q.lo[next], o);
+  const unsigned n = decode_seq<true>(S, sc.bits, p, z, c, q.lo[i + 1], b, b_end, q.lo[next], o);
   if (next == i + 1 && b + n < b_end) *o.err = 1;  // the interval holds fewer blocks than it must
-}
-__global__ void __launch_bounds__(128) k_hd_write(const uint32_t* __restrict__ bits, const unsigned long long* __restrict__ out, const unsigned* __restrict__ base,
-                                                  const HdShared* __restrict__ gs, const HdSeqs q, HdOut o) {
-  __shared__ HdShared S;
-  stage_shared(S, gs);
-  hd_write_seq(S, blockIdx.x * blockDim.x + threadIdx.x, bits, out, base, q, o);
-}
-
-// ---- a batch of scans (jpeg_entropy_decode_batch_dev) ----
-// Scan s owns subsequence slots [seq0, seq0 + nseq + 1) of the batch's per-subsequence arrays, seq0 a multiple of
-// 128, so that every CTA of the relaxation and writing passes works on one scan and stages one scan's tables; and
-// intervals [iv0, iv0 + nint + 1) of its per-interval arrays.  Within its slice a scan is laid out as alone.
-struct HdScan {
-  const uint32_t* bits;
-  unsigned seq0, iv0, nint;
-  HdOut o;
-};
-struct HdBatch {
-  const HdShared* gs;     // per scan
-  const HdScan* scans;
-  const uint2* ctas;      // per CTA of a launch: {scan, first slot}
-  const unsigned* start;  // per interval: start bit (local to the scan)
-  HdSeqs q;               // lo / iv / first of every scan, values local to the scan
-};
-__device__ __forceinline__ HdSeqs hd_local(const HdBatch& B, const HdScan& sc) {
-  return HdSeqs{B.q.lo + sc.seq0, B.q.iv + sc.seq0, B.q.first + sc.iv0};
-}
-
-// k_hd_layout and k_hd_init of every scan in one launch, one thread per slot
-__global__ void __launch_bounds__(128) k_hd_layout_batch(const HdBatch B, unsigned* lo, unsigned* iv, unsigned long long* out,
-                                                         unsigned long long* used, unsigned* cnt) {
-  const uint2 cta = B.ctas[blockIdx.x];
-  const HdScan& sc = B.scans[cta.x];
-  const unsigned nseq = B.gs[cta.x].f.nseq, total_bits = B.gs[cta.x].f.total_bits;
-  const unsigned i = cta.y - sc.seq0 + threadIdx.x;
-  const HdSeqs q = hd_local(B, sc);
-  const unsigned* start = B.start + sc.iv0;
-  if (i == 0) lo[sc.seq0 + nseq] = total_bits;
-  if (i >= nseq) return;
-  unsigned iv1;
-  lo[sc.seq0 + i] = hd_seq_lo(start, q.first, sc.nint, i, iv + sc.seq0 + i);
-  out[sc.seq0 + i] = i + 1 < nseq ? (unsigned long long)hd_seq_lo(start, q.first, sc.nint, i + 1, &iv1) : (unsigned long long)total_bits;
-  used[sc.seq0 + i] = ~0ull;
-  cnt[sc.seq0 + i] = 0;
-}
-
-// one relaxation round over the CTAs of the scans that still need rounds; a scan's change stores round + 1 into
-// last[scan]
-__global__ void __launch_bounds__(128) k_hd_sync_batch(const HdBatch B, unsigned long long* out, unsigned long long* used, unsigned* cnt,
-                                                       unsigned* last, const unsigned round) {
-  __shared__ HdShared S;
-  const uint2 cta = B.ctas[blockIdx.x];
-  const HdScan& sc = B.scans[cta.x];
-  const unsigned seq0 = sc.seq0;
-  hd_sync_seq(S, cta.y - seq0 + threadIdx.x, sc.bits, out + seq0, used + seq0, cnt + seq0, last + cta.x, round + 1, B.gs + cta.x,
-              hd_local(B, sc));
-}
-
-// k_hd_scan of each scan that had rounds: one CTA per scan
-__global__ void __launch_bounds__(1024) k_hd_scan_batch(const HdBatch B, const unsigned* __restrict__ which, const unsigned* __restrict__ cnt,
-                                                        unsigned* __restrict__ base) {
-  const unsigned s = which[blockIdx.x];
-  const unsigned seq0 = B.scans[s].seq0;
-  hd_prefix(cnt + seq0, base + seq0, B.gs[s].f.nseq);
-}
-
-__global__ void __launch_bounds__(128) k_hd_write_batch(const HdBatch B, const unsigned long long* __restrict__ out,
-                                                        const unsigned* __restrict__ base) {
-  __shared__ HdShared S;
-  const uint2 cta = B.ctas[blockIdx.x];
-  stage_shared(S, B.gs + cta.x);
-  const HdScan& sc = B.scans[cta.x];
-  const unsigned seq0 = sc.seq0;
-  hd_write_seq(S, cta.y - seq0 + threadIdx.x, sc.bits, out + seq0, base + seq0, hd_local(B, sc), sc.o);
 }
 
 // ---- DC prediction: inclusive scan of the differences per component, scatter into the blocks ----
@@ -397,17 +359,27 @@ __device__ __forceinline__ int cta_inclusive_scan(int v, int* warp_sums /* [32] 
   __syncthreads();
   return x + ((threadIdx.x >> 5) ? warp_sums[(threadIdx.x >> 5) - 1] : 0);
 }
-__device__ __forceinline__ void dc_local(const DcPlan& d, const unsigned cta) {
+
+// The three DC passes over many plans (every component of every scan of a batch), one launch each.  cta_end[j]: the
+// CTAs of plans 0..j in the launch's numbering (inclusive prefix), kDcCta-thread CTAs for the local pass, 256-thread
+// ones for the scatter; the sums pass runs one CTA per plan.
+__global__ void __launch_bounds__(kDcCta) k_dc_local(const DcPlan* __restrict__ plans, const unsigned* __restrict__ cta_end, unsigned n) {
   __shared__ int ws[32];
+  const unsigned j = batch_find(cta_end, n, blockIdx.x);
+  const DcPlan& d = plans[j];
+  const unsigned cta = blockIdx.x - (j ? cta_end[j - 1] : 0);
   const unsigned i = cta * kDcCta + threadIdx.x;
   const int x = cta_inclusive_scan(i < d.n ? d.dcd[i] : 0, ws);
   if (i < d.n) d.dcd[i] = x;
   if (threadIdx.x == kDcCta - 1) d.sums[cta] = x;
 }
-__global__ void __launch_bounds__(kDcCta) k_dc_local(DcPlan d) { dc_local(d, blockIdx.x); }
-__device__ __forceinline__ void dc_sums(int* sums, unsigned n) {  // in place, exclusive, one CTA
+// each plan's per-CTA totals, in place, exclusive
+__global__ void __launch_bounds__(kDcCta) k_dc_sums(const DcPlan* __restrict__ plans) {
   __shared__ int ws[32];
   __shared__ int carry;
+  const DcPlan& d = plans[blockIdx.x];
+  int* sums = d.sums;
+  const unsigned n = (d.n + kDcCta - 1) / kDcCta;
   if (threadIdx.x == 0) carry = 0;
   __syncthreads();
   for (unsigned start = 0; start < n; start += kDcCta) {
@@ -420,8 +392,10 @@ __device__ __forceinline__ void dc_sums(int* sums, unsigned n) {  // in place, e
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(kDcCta) k_dc_sums(int* sums, unsigned n) { dc_sums(sums, n); }
-__device__ __forceinline__ void dc_apply(const DcPlan& d, const unsigned i) {
+__global__ void __launch_bounds__(256) k_dc_apply(const DcPlan* __restrict__ plans, const unsigned* __restrict__ cta_end, unsigned n) {
+  const unsigned j = batch_find(cta_end, n, blockIdx.x);
+  const DcPlan& d = plans[j];
+  const unsigned i = (blockIdx.x - (j ? cta_end[j - 1] : 0)) * 256 + threadIdx.x;
   if (i >= d.n) return;
   // running sum within the interval = prefix sum to i minus prefix sum before the interval's first block;
   // exact in wrapping 32-bit arithmetic, which is how jpeg_host_decode_coefs accumulates too
@@ -432,23 +406,6 @@ __device__ __forceinline__ void dc_apply(const DcPlan& d, const unsigned i) {
   const int bx = (int)(mcu % (unsigned)d.mcus_per_row) * d.h + (int)(k % (unsigned)d.h);
   const int by = (int)(mcu / (unsigned)d.mcus_per_row) * d.v + (int)(k / (unsigned)d.h);
   if (bx < d.wblocks && by < d.hblocks) d.coefs[((size_t)by * d.wblocks + bx) * 64] = (int16_t)dc;
-}
-__global__ void __launch_bounds__(256) k_dc_apply(DcPlan d) { dc_apply(d, blockIdx.x * blockDim.x + threadIdx.x); }
-
-// The three DC passes over many plans (every component of every scan of a batch), one launch each.  cta_end[j]: the
-// CTAs of plans 0..j in the launch's numbering (inclusive prefix), kDcCta-thread CTAs for the local pass, 256-thread
-// ones for the scatter; the sums pass runs one CTA per plan.
-__global__ void __launch_bounds__(kDcCta) k_dc_local_batch(const DcPlan* __restrict__ plans, const unsigned* __restrict__ cta_end, unsigned n) {
-  const unsigned j = batch_find(cta_end, n, blockIdx.x);
-  dc_local(plans[j], blockIdx.x - (j ? cta_end[j - 1] : 0));
-}
-__global__ void __launch_bounds__(kDcCta) k_dc_sums_batch(const DcPlan* __restrict__ plans) {
-  const DcPlan& d = plans[blockIdx.x];
-  dc_sums(d.sums, (d.n + kDcCta - 1) / kDcCta);
-}
-__global__ void __launch_bounds__(256) k_dc_apply_batch(const DcPlan* __restrict__ plans, const unsigned* __restrict__ cta_end, unsigned n) {
-  const unsigned j = batch_find(cta_end, n, blockIdx.x);
-  dc_apply(plans[j], (blockIdx.x - (j ? cta_end[j - 1] : 0)) * 256 + threadIdx.x);
 }
 
 void build_tables(const JpegHeader& h, HdTables* t) {
@@ -481,9 +438,9 @@ void build_tables(const JpegHeader& h, HdTables* t) {
 
 namespace {
 std::atomic<unsigned long long> g_hd_done{0}, g_hd_declined{0}, g_hd_rounds{0};
-int declined() {
+bool declined() {
   g_hd_declined.fetch_add(1);
-  return kHuffDecFallback;
+  return false;
 }
 }  // namespace
 void jpeg_entropy_decoder_stats(unsigned long long out[3]) {
@@ -528,8 +485,8 @@ static long unstuff_scan(const uint8_t* data, size_t size, size_t from, uint8_t*
 }
 
 // The frame description and tables of a scan (all of hs but total_bits and nseq), its MCUs per restart interval and
-// its intervals; kHuffDecFallback for a scan the device decoder does not take
-static int hd_prepare(const JpegHeader& h, HdShared& hs, size_t* ri_out, unsigned* nint_out) {
+// its intervals; false for a scan the device decoder does not take
+static bool hd_prepare(const JpegHeader& h, HdShared& hs, size_t* ri_out, unsigned* nint_out) {
   const JpegFrame& f = h.frame;
   memset(&hs, 0, sizeof hs);
   HdFrame& hf = hs.f;
@@ -569,7 +526,7 @@ static int hd_prepare(const JpegHeader& h, HdShared& hs, size_t* ri_out, unsigne
   build_tables(h, &hs.t);
   *ri_out = ri;
   *nint_out = nint;
-  return E_OK;
+  return true;
 }
 
 // subsequences: every interval is cut into pieces of at most kSeqBits bits (an empty interval gets one empty piece,
@@ -593,153 +550,18 @@ static int upload_zigzag() {
   return device_table(zigzag, 64, [](void* host) { memcpy(host, kZigzag, 64); }, &kZigzagDev) ? E_OK : E_ERROR;
 }
 
-int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, const JpegHeader& h, int16_t* d_coefs[3]) {
-  const JpegFrame& f = h.frame;
-  HdShared hs;
-  HdFrame& hf = hs.f;
-  size_t ri = 0;
-  unsigned nint = 0;
-  if (int rc = hd_prepare(h, hs, &ri, &nint)) return rc;
-  const size_t mcus = (size_t)f.mcus_per_row * f.mcu_rows;
-
-  // 1. clean bit stream in pinned memory, then on the device (8 zero bytes of slack for the reader)
-  if (size <= h.scan_offset) return fail(E_ERROR, "Corrupt JPEG data: no entropy-coded segment");
-  const size_t cap = size - h.scan_offset + 16;
-  uint8_t* h_bits = (uint8_t*)ws.halloc(cap);
-  unsigned* h_starts = (unsigned*)ws.halloc(sizeof(unsigned) * nint);
-  if (!h_bits || !h_starts) return E_MEM;
-  PhaseTrace tr;
-  const long clean = unstuff_scan(data, size, h.scan_offset, h_bits, h.restart_interval != 0, h_starts, nint);
-  tr.mark("  unstuff");
-  if (clean < 0) return declined();
-  if ((size_t)clean * 8 > 0xfffffff0u - kSeqBits) return declined();
-  memset(h_bits + clean, 0, 16);
-  const size_t padded = ((size_t)clean + 16 + 3) & ~(size_t)3;
-  hf.total_bits = (unsigned)(clean * 8);
-  if (hf.total_bits == 0) return fail(E_ERROR, "Corrupt JPEG data: empty entropy-coded segment");
-
-  unsigned* h_first = (unsigned*)ws.halloc(sizeof(unsigned) * (nint + 1));
-  if (!h_first) return E_MEM;
-  const unsigned nseq = hd_intervals(h_starts, h_first, nint, hf.total_bits);
-  hf.nseq = nseq;
-  tr.mark("  interval layout");
-
-  uint32_t* d_bits = (uint32_t*)ws.dalloc(padded);
-  HdShared* d_hs = (HdShared*)ws.dalloc(sizeof(HdShared));
-  HdShared* h_hs = (HdShared*)ws.halloc(sizeof(HdShared));
-  unsigned long long* d_out = (unsigned long long*)ws.dalloc(sizeof(unsigned long long) * nseq);
-  unsigned long long* d_used = (unsigned long long*)ws.dalloc(sizeof(unsigned long long) * nseq);
-  unsigned* d_cnt = (unsigned*)ws.dalloc(sizeof(unsigned) * nseq);
-  unsigned* d_base = (unsigned*)ws.dalloc(sizeof(unsigned) * nseq);
-  unsigned* d_flags = (unsigned*)ws.dalloc(sizeof(unsigned) * (kMaxRounds + 8));
-  unsigned* h_flags = (unsigned*)ws.halloc(sizeof(unsigned) * (kMaxRounds + 8));
-  unsigned* d_start = (unsigned*)ws.dalloc(sizeof(unsigned) * nint);
-  unsigned* d_first = (unsigned*)ws.dalloc(sizeof(unsigned) * (nint + 1));
-  unsigned* d_lo = (unsigned*)ws.dalloc(sizeof(unsigned) * (nseq + 1));
-  unsigned* d_iv = (unsigned*)ws.dalloc(sizeof(unsigned) * nseq);
-  if (!d_bits || !d_hs || !h_hs || !d_out || !d_used || !d_cnt || !d_base || !d_flags || !h_flags || !d_start || !d_first || !d_lo || !d_iv)
-    return E_MEM;
-  const HdSeqs q = {d_lo, d_iv, d_first};
-  memcpy(h_hs, &hs, sizeof hs);
-  cudaStream_t s = ws.stream();
-  CUDA_TRY(cudaMemcpyAsync(d_bits, h_bits, padded, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(d_hs, h_hs, sizeof hs, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(d_start, h_starts, sizeof(unsigned) * nint, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(d_first, h_first, sizeof(unsigned) * (nint + 1), cudaMemcpyHostToDevice, s));
-  k_hd_layout<<<(nseq + 255) / 256, 256, 0, s>>>(d_start, d_first, nint, nseq, hf.total_bits, d_lo, d_iv);
-  count_launches(1);
-  CUDA_TRY(cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (kMaxRounds + 8), s));
-  if (int rc = upload_zigzag()) return rc;
-  // coefficient blocks start as zeros; only non-zero coefficients are written
-  int* d_dcd[3] = {nullptr, nullptr, nullptr};
-  for (int c = 0; c < f.ncomp; c++) {
-    d_coefs[c] = (int16_t*)ws.dalloc(f.blocks(c) * 128);
-    d_dcd[c] = (int*)ws.dalloc(sizeof(int) * mcus * hf.hv[c]);
-    if (!d_coefs[c] || !d_dcd[c]) return E_MEM;
-    CUDA_TRY(cudaMemsetAsync(d_coefs[c], 0, f.blocks(c) * 128, s));
-  }
-
-  // 2. relaxation rounds until one of them changes nothing; none when every subsequence starts an
-  // interval, since all entry states are then known
-  const unsigned grid = (nseq + 127) / 128;
-  const bool relax = nseq > nint;
-  int rounds = 0, first_quiet = 0;
-  if (relax) {
-    ws.t_begin("huffdec_sync");
-    k_hd_init<<<(nseq + 255) / 256, 256, 0, s>>>(d_out, d_used, d_cnt, nseq, q.lo);
-    count_launches(1);
-    bool converged = false;
-    while (!converged && rounds < kMaxRounds) {
-      count_launches(kRoundsPerBatch);
-      for (int r = 0; r < kRoundsPerBatch; r++) k_hd_sync<<<grid, 128, 0, s>>>(d_bits, d_out, d_used, d_cnt, d_flags + rounds + r, d_hs, q);
-      CUDA_TRY(cudaGetLastError());
-      CUDA_TRY(cudaMemcpyAsync(h_flags + rounds, d_flags + rounds, sizeof(unsigned) * kRoundsPerBatch, cudaMemcpyDeviceToHost, s));
-      CUDA_TRY(cudaStreamSynchronize(s));
-      for (int r = 0; r < kRoundsPerBatch && !converged; r++)
-        if (!h_flags[rounds + r]) {
-          converged = true;
-          first_quiet = rounds + r + 1;
-        }
-      rounds += kRoundsPerBatch;
-    }
-    ws.t_end();
-    tr.mark("  relaxation rounds");
-    if (!converged) return declined();
-  }
-
-  // 3. block offsets within each interval, then the writing pass
-  unsigned* d_err = d_flags + kMaxRounds;
-  HdOut o;
-  memset(&o, 0, sizeof o);
-  for (int c = 0; c < f.ncomp; c++) { o.coefs[c] = d_coefs[c]; o.dcd[c] = d_dcd[c]; }
-  o.err = d_err;
-  ws.t_begin("huffdec_write");
-  count_launches((relax ? 2 : 1) + 3 * f.ncomp);
-  if (relax) k_hd_scan<<<1, 1024, 0, s>>>(d_cnt, d_base, nseq);
-  k_hd_write<<<grid, 128, 0, s>>>(d_bits, d_out, d_base, d_hs, q, o);
-  ws.t_end();
-  CUDA_TRY(cudaGetLastError());
-  // 4. DC prediction
-  ws.t_begin("huffdec_dc");
-  for (int c = 0; c < f.ncomp; c++) {
-    DcPlan d;
-    d.dcd = d_dcd[c];
-    d.coefs = d_coefs[c];
-    d.n = (unsigned)(mcus * hf.hv[c]);
-    d.seg = (unsigned)(ri * hf.hv[c]);
-    d.h = hf.h[c]; d.v = hf.v[c]; d.hv = hf.hv[c];
-    d.wblocks = hf.wblocks[c]; d.hblocks = hf.hblocks[c];
-    d.mcus_per_row = hf.mcus_per_row;
-    const unsigned nct = (d.n + kDcCta - 1) / kDcCta;
-    d.sums = (int*)ws.dalloc(sizeof(int) * nct);
-    if (!d.sums) return E_MEM;
-    k_dc_local<<<nct, kDcCta, 0, s>>>(d);
-    k_dc_sums<<<1, kDcCta, 0, s>>>(d.sums, nct);
-    k_dc_apply<<<(d.n + 255) / 256, 256, 0, s>>>(d);
-  }
-  ws.t_end();
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(h_flags, d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  tr.mark("  write + dc");
-  if (h_flags[0]) return declined();  // let the host decoder produce the diagnosis
-  g_hd_done.fetch_add(1);
-  g_hd_rounds.store((unsigned long long)first_quiet);
-  return E_OK;
-}
-
 namespace {
 template <typename T>
 T* dalloc_n(Workspace& ws, size_t n) { return (T*)ws.dalloc(sizeof(T) * (n ? n : 1)); }
 template <typename T>
 T* halloc_n(Workspace& ws, size_t n) { return (T*)ws.halloc(sizeof(T) * (n ? n : 1)); }
-void scan_error(JpegBatchScan& sc, int rc) {
+void scan_error(JpegScanJob& sc, int rc) {
   sc.rc = rc;
   snprintf(sc.err, sizeof sc.err, "%s", last_error());
 }
 }  // namespace
 
-int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
+int jpeg_entropy_decode_dev(Workspace& ws, JpegScanJob* scans, int n) {
   cudaStream_t s = ws.stream();
   struct Plan {
     bool dev;              // on the device (else the host decoder)
@@ -750,16 +572,19 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
   Plan* pl = halloc_n<Plan>(ws, n);
   HdShared* h_hs = halloc_n<HdShared>(ws, n);
   if (!pl || !h_hs) return E_MEM;
-  // 1. per scan, on the host: tables, intervals, and the staging size of its clean bits
+  PhaseTrace tr;
+  // 1. per scan, on the host: tables, intervals, and the staging size of its clean bits.  With the host decoder
+  // selected (jpeg_set_entropy_decoder(1)) every scan goes to it, and the device decoder's counts do not move.
+  const bool host_only = jpeg_get_entropy_decoder() == 1;
   size_t bits_cap = 0, niv = 0;
   for (int i = 0; i < n; i++) {
-    JpegBatchScan& sc = scans[i];
+    JpegScanJob& sc = scans[i];
     const JpegHeader& h = *sc.h;
     Plan& p = pl[i];
     memset(&p, 0, sizeof p);
     sc.rc = E_OK;
     for (int c = 0; c < 3; c++) sc.d_coefs[c] = nullptr;
-    p.dev = hd_prepare(h, h_hs[i], &p.ri, &p.nint) == E_OK;
+    p.dev = !host_only && hd_prepare(h, h_hs[i], &p.ri, &p.nint);
     if (!p.dev) continue;
     if (sc.size <= h.scan_offset) {
       scan_error(sc, fail(E_ERROR, "Corrupt JPEG data: no entropy-coded segment"));
@@ -777,7 +602,7 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
   // 2. every scan unstuffed into one pinned buffer; a scan with irregular restart markers goes to the host decoder
   size_t nslots = 0, nrelax = 0, cta_all = 0, cta_sync = 0;
   for (int i = 0; i < n; i++) {
-    JpegBatchScan& sc = scans[i];
+    JpegScanJob& sc = scans[i];
     Plan& p = pl[i];
     if (!p.dev || sc.rc) continue;
     uint8_t* dst = h_bits + p.bits_off;
@@ -805,6 +630,7 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
       nrelax++;
     }
   }
+  tr.mark("  unstuff");
   if (nslots > 0xffffff00u) return fail(E_ERROR, "internal: entropy-decoder batch of %zu subsequences", nslots);
   // the CTA lists (all scans, then those with rounds), the scans with rounds, the per-scan slices, the DC plans
   uint2* h_ctas = halloc_n<uint2>(ws, cta_all + cta_sync);
@@ -837,7 +663,7 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
   // blocks are copied over them)
   size_t a = 0, b = 0, nw = 0, ndc = 0, n_local = 0, n_apply = 0;
   for (int i = 0; i < n; i++) {
-    JpegBatchScan& sc = scans[i];
+    JpegScanJob& sc = scans[i];
     const Plan& p = pl[i];
     if (sc.rc) continue;
     const JpegFrame& f = sc.h->frame;
@@ -897,20 +723,21 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
     CUDA_TRY(cudaMemsetAsync(d_last, 0, sizeof(unsigned) * 2 * n, s));
     if (int rc = upload_zigzag()) return rc;
     HdBatch B = {d_hs, d_scans, d_ctas, d_start, HdSeqs{d_lo, d_iv, d_first}};
-    k_hd_layout_batch<<<(unsigned)cta_all, 128, 0, s>>>(B, d_lo, d_iv, d_out, d_used, d_cnt);
+    k_hd_layout<<<(unsigned)cta_all, 128, 0, s>>>(B, d_lo, d_iv, d_out, d_used, d_cnt);
     count_launches(1);
     CUDA_TRY(cudaGetLastError());
+    tr.mark("  interval layout");
     // 3. relaxation rounds over every scan that has them, one host check per kRoundsPerBatch rounds for the whole
     // batch, until each of them has had a round that changed nothing
     int rounds = 0;
     bool pending = cta_sync > 0;
     HdBatch Bs = B;
     Bs.ctas = d_ctas + cta_all;
-    if (pending) ws.t_begin("huffdec_sync_batch");
+    if (pending) ws.t_begin("huffdec_sync");
     while (pending && rounds < kMaxRounds) {
       count_launches(kRoundsPerBatch);
       for (int r = 0; r < kRoundsPerBatch; r++)
-        k_hd_sync_batch<<<(unsigned)cta_sync, 128, 0, s>>>(Bs, d_out, d_used, d_cnt, d_last, (unsigned)(rounds + r));
+        k_hd_sync<<<(unsigned)cta_sync, 128, 0, s>>>(Bs, d_out, d_used, d_cnt, d_last, (unsigned)(rounds + r));
       CUDA_TRY(cudaGetLastError());
       CUDA_TRY(cudaMemcpyAsync(h_last, d_last, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, s));
       CUDA_TRY(cudaStreamSynchronize(s));
@@ -918,30 +745,32 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
       pending = false;
       for (size_t j = 0; j < nrelax; j++) pending = pending || h_last[h_which[j]] == (unsigned)rounds;  // changed in the last round
     }
-    if (cta_sync) ws.t_end();
+    if (cta_sync) {
+      ws.t_end();
+      tr.mark("  relaxation rounds");
+    }
     for (size_t j = 0; j < nrelax; j++) {
       const unsigned i = h_which[j];
       if (h_last[i] == (unsigned)rounds) {  // no quiet round in kMaxRounds: the host decoder takes it
         pl[i].dev = false;
         declined();
-      } else {
-        g_hd_rounds.store((unsigned long long)h_last[i] + 1);  // the first quiet round
       }
     }
     // 4. block offsets within each interval, the writing pass, DC prediction: one launch each for the batch
-    ws.t_begin("huffdec_write_batch");
-    if (nrelax) k_hd_scan_batch<<<(unsigned)nrelax, 1024, 0, s>>>(B, d_which, d_cnt, d_base);
-    k_hd_write_batch<<<(unsigned)cta_all, 128, 0, s>>>(B, d_out, d_base);
+    ws.t_begin("huffdec_write");
+    if (nrelax) k_hd_scan<<<(unsigned)nrelax, 1024, 0, s>>>(B, d_which, d_cnt, d_base);
+    k_hd_write<<<(unsigned)cta_all, 128, 0, s>>>(B, d_out, d_base);
     ws.t_end();
-    ws.t_begin("huffdec_dc_batch");
-    k_dc_local_batch<<<(unsigned)n_local, kDcCta, 0, s>>>(d_dc, d_dc_end, (unsigned)ndc);
-    k_dc_sums_batch<<<(unsigned)ndc, kDcCta, 0, s>>>(d_dc);
-    k_dc_apply_batch<<<(unsigned)n_apply, 256, 0, s>>>(d_dc, d_dc_end + 3 * n, (unsigned)ndc);
+    ws.t_begin("huffdec_dc");
+    k_dc_local<<<(unsigned)n_local, kDcCta, 0, s>>>(d_dc, d_dc_end, (unsigned)ndc);
+    k_dc_sums<<<(unsigned)ndc, kDcCta, 0, s>>>(d_dc);
+    k_dc_apply<<<(unsigned)n_apply, 256, 0, s>>>(d_dc, d_dc_end + 3 * n, (unsigned)ndc);
     ws.t_end();
     count_launches((nrelax ? 1 : 0) + 4);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(h_last + n, d_last + n, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
+    tr.mark("  write + dc");
     for (int i = 0; i < n; i++) {
       if (!pl[i].dev || scans[i].rc) continue;
       if (h_last[n + i]) {  // let the host decoder produce the diagnosis
@@ -949,12 +778,13 @@ int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n) {
         declined();
       } else {
         g_hd_done.fetch_add(1);
+        g_hd_rounds.store(pl[i].relax ? (unsigned long long)h_last[i] + 1 : 0ull);  // the first quiet round
       }
     }
   }
   // 5. the scans the device decoder did not take, on the host; their blocks replace the device's
   for (int i = 0; i < n; i++) {
-    JpegBatchScan& sc = scans[i];
+    JpegScanJob& sc = scans[i];
     if (pl[i].dev || sc.rc) continue;
     const JpegFrame& f = sc.h->frame;
     int16_t* h_coefs[3] = {nullptr, nullptr, nullptr};

@@ -156,18 +156,13 @@ int jpeg_idct_dev(Workspace& ws, const JpegIdctJob* jobs, int n);
 // One k_idct<0> launch over planes[0, n) of a jpeg_idct_stage, after one copy to the device: each plane's coefficients
 // are read once and written at every size its outputs ask for
 int jpeg_idct_multi_dev(Workspace& ws, IdctPlane* planes, int n);
-// Entropy decoding on the device (huffdec.cu): fills d_coefs[c] (allocated from the workspace) with
-// [block][64] natural-order coefficients.  Returns kHuffDecFallback when the stream is outside what
-// the parallel decoder handles (restart markers, no fixed point, inconsistent data): the caller then
-// runs jpeg_host_decode_coefs, which also produces the reference's error texts.
-constexpr int kHuffDecFallback = -1000;
-int jpeg_entropy_decode_dev(Workspace& ws, const uint8_t* data, size_t size, const JpegHeader& h, int16_t* d_coefs[3]);
-// Entropy decoding of many JPEGs at once: one relaxation over the subsequences of every scan (one host check per
-// batch of rounds for all of them), then one writing pass and one DC pass.  The coefficients are those
-// jpeg_entropy_decode_dev, or the host decoder where it declines, gives for each JPEG alone; a scan the device decoder
-// declines goes to jpeg_host_decode_coefs by itself.  Enqueued on ws.stream(), the last copies may still be in flight.
-// Returns an error only for what fails the whole batch (CUDA, memory); a corrupt scan gets its code in rc.
-struct JpegBatchScan {
+// Entropy decoding (huffdec.cu) of one or many JPEGs: one relaxation over the subsequences of every scan (one host
+// check per batch of rounds for all of them), then one writing pass and one DC pass.  A scan the device decoder
+// declines (irregular restart markers, no fixed point, inconsistent data), and every scan while the host decoder is
+// selected, goes to jpeg_host_decode_coefs by itself; that decoder also produces the reference's error texts.
+// Enqueued on ws.stream(), the last copies may still be in flight.  Returns an error only for what fails the whole
+// call (CUDA, memory); a corrupt scan gets its code in rc.
+struct JpegScanJob {
   const uint8_t* data;
   size_t size;
   const JpegHeader* h;
@@ -175,7 +170,7 @@ struct JpegBatchScan {
   int rc;               // out: E_OK, or the error decoding this scan gives (its message in err)
   char err[256];
 };
-int jpeg_entropy_decode_batch_dev(Workspace& ws, JpegBatchScan* scans, int n);
+int jpeg_entropy_decode_dev(Workspace& ws, JpegScanJob* scans, int n);
 // 0 = default = 2 = device whenever the stream allows (host only for streams the device decoder declines), 1 = host (tests, triage)
 // [0] scans decoded on the device, [1] scans handed back to the host decoder, [2] relaxation rounds of the last one
 void jpeg_entropy_decoder_stats(unsigned long long out[3]);

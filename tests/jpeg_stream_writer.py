@@ -8,7 +8,7 @@ gives the clean (unstuffed) bit offset, kind and scan block of every symbol, so 
 boundary exactly where it wants.
 
 Model: `Decoder.decode` is decode_seq of huffdec.cu over the clean bits (same tables, same handling of codes that are
-not in the table), `relax_rounds` replays k_hd_init + k_hd_sync rounds in lock step (each round reads only the
+not in the table), `relax_rounds` replays k_hd_layout + k_hd_sync rounds in lock step (each round reads only the
 states of the round before), and `flat_phases` lists the bit phases of a repeating flat MCU from which a decoder
 started in the first-guess state (DC symbol of block 0 next) never falls back into step.
 """
@@ -414,7 +414,7 @@ def subsequences(st):
 
 
 def relax_rounds(st, max_rounds=MAX_ROUNDS):
-    """k_hd_init + k_hd_sync in lock step -> (first round that changes nothing, or None if none within
+    """k_hd_layout + k_hd_sync in lock step -> (first round that changes nothing, or None if none within
     max_rounds; 0 when every subsequence starts an interval; subsequences; per round the subsequences it changed)"""
     seqs = subsequences(st)
     n = len(seqs)

@@ -196,6 +196,32 @@ def test_flat_scan_goes_to_the_host_decoder_alone(lib):
         assert same(it.result(), w)
 
 
+
+def test_host_decoder_switch_applies_to_batches(lib):
+    """uhdr_b200_set_entropy_decoder(1) sends every scan of a batch to the host decoder: the same pixels and codes as
+    the device decoder gives, and the device decoder's counts do not move"""
+    good = files(lib, 1)
+    datas = [good[0], corrupt_file(lib, good[0]), good[6], good[8], good[9]]
+    runs = {}
+    for mode in (2, 1):
+        prev = lib.uhdr_b200_set_entropy_decoder(mode)
+        try:
+            items = [Item(lib, d, 1, A.FMT_RGBAF16) for d in datas]
+            s0 = _stats(lib)
+            rc, st = batch(lib, items, 1, A.CT_LINEAR, 4.0)
+            torch().cuda.synchronize()
+            s1 = _stats(lib)
+        finally:
+            lib.uhdr_b200_set_entropy_decoder(prev)
+        runs[mode] = (rc, st, lib.uhdr_b200_last_error(), items, (s1[0] - s0[0], s1[1] - s0[1]))
+    rc, st, err, items, dev = runs[2]
+    assert st == [0, rc, 0, 0, 0] and rc != 0, (rc, st, err)
+    assert runs[1][:3] == (rc, st, err)
+    assert items[1].untouched() and runs[1][3][1].untouched()
+    for a, b in zip(items, runs[1][3]):
+        assert same(a.result(), b.result())
+    assert dev[0] > 0 and runs[1][4] == (0, 0), (dev, runs[1][4])
+
 def corrupt_file(lib, data):
     """data with bytes of the primary image's entropy-coded segment overwritten so that decoding it fails (not every
     damage does: some decode to other pixels), found by trying seeded damages"""

@@ -1,5 +1,5 @@
-"""The GPU JPEG decoder route by route (huffdec.cu k_hd_sync / k_hd_scan / k_hd_write / k_dc_*, then k_idct<8>
-and k_ycc_to_rgba) on streams other encoders write: optimised and hand-made Huffman tables, every table selector,
+"""The GPU JPEG decoder route by route (huffdec.cu k_hd_layout / k_hd_sync / k_hd_scan / k_hd_write / k_dc_*, then
+k_idct<8> and k_ycc_to_rgba) on streams other encoders write: optimised and hand-made Huffman tables, every table selector,
 4:4:0 / 4:1:1 / 4:1:0 and 10-block MCUs, subsequence boundaries on every bit of a symbol, restart intervals of
 n 1024 +- 1 bits, flat frames whose relaxation converges slowly or not at all, IDCT and colour-conversion edges.
 

@@ -204,6 +204,27 @@ def test_scan_handed_back_to_the_host(lib, corpus):
     _check_batch(lib, datas, 2, 60, 90, 1, 1)
 
 
+
+def test_host_decoder_switch_applies_to_batches(lib, corpus):
+    """uhdr_b200_set_entropy_decoder(1) sends every scan of a batch to the host decoder: the same bytes, sizes and
+    codes as the device decoder gives, and the device decoder's counts do not move"""
+    garbage = b"\xff\xd8\xff\xe0" + bytes(range(200)) + b"\xff\xd9"
+    datas = [corpus["own_api1_420_rgbmap"], corpus["foreign_tables_restart"], garbage, corpus["pgray"],
+             corpus["apple_gainmap_new.jpg"]]
+    runs = {}
+    for mode in (2, 1):
+        prev = lib.uhdr_b200_set_entropy_decoder(mode)
+        try:
+            s0 = _dec_stats(lib)
+            rc, got = batch(lib, datas, 2, 75, 60, 1, 1)
+            s1 = _dec_stats(lib)
+        finally:
+            lib.uhdr_b200_set_entropy_decoder(prev)
+        runs[mode] = (rc, got, lib.uhdr_b200_last_error(), (s1[0] - s0[0], s1[1] - s0[1]))
+    assert [g[0] for g in runs[2][1]] == [0, 0, runs[2][0], 0, 0] and runs[2][0] != 0, runs[2][:3]
+    assert runs[1][:3] == runs[2][:3]
+    assert runs[2][3][0] > 0 and runs[1][3] == (0, 0), (runs[2][3], runs[1][3])
+
 def test_groups_give_the_same_bytes(lib, corpus, monkeypatch):
     datas = list(corpus.values())
     _rc, whole = batch(lib, datas, 2, 75, 75, 1, 1)
