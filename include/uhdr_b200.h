@@ -307,6 +307,33 @@ typedef struct uhdr_b200_transcode_rung {
   int status;                        /* out: this rung's uhdr_codec_err_t */
 } uhdr_b200_transcode_rung_t;
 UHDR_EXTERN int uhdr_b200_transcode_ladder(const void* data, size_t size, uhdr_b200_transcode_rung_t* rungs, int n);
+/* uhdr_b200_transcode_ladder over MANY files in one call, each file with its own ladder (a derivative set for every
+ * upload): the files are taken in groups, and per group both JPEGs of every file are entropy-decoded once, one inverse
+ * DCT pass writes every reduced size every file's rungs ask for, and all the group's rungs share one staging pass, one
+ * block stage per distinct (base_quality, gainmap_quality) pair and one entropy coding, with two host waits.
+ *  - Each file gets exactly what uhdr_b200_transcode_ladder(data, size, rungs, n) gives for it alone: that return value
+ *    in status, and on every rung the same bytes, out_size and status.  So every rung equals uhdr_b200_transcode with
+ *    its cfg alone.  A file's null data or rungs, or n outside 1..16, give UHDR_CODEC_INVALID_PARAM on that file and
+ *    touch none of its rungs.  A failing file or rung writes nothing; the others are unaffected.
+ *  - A null files or n < 1 give UHDR_CODEC_INVALID_PARAM and touch no file.  Otherwise the return value is
+ *    UHDR_CODEC_OK when every file succeeded, else the first failing file's status, and uhdr_b200_last_error() reads
+ *    "file <i>: <that ladder's message>" ("file <i>: rung <j>: ..." for an error of a rung).  An error of the whole
+ *    call (CUDA, device memory) ends it and is set as the status of every file and rung without an error of its own.
+ *    Without a device: UHDR_CODEC_ERROR with a CUDA message on every valid rung, as uhdr_b200_transcode_ladder gives.
+ *  - A group closes before its scratch would exceed a device-memory budget (4 GiB; the environment variable
+ *    UHDR_B200_BATCH_GROUP_BYTES sets another), 2^29 entropy-coded bytes or 16 distinct quality pairs; a file is never
+ *    split, and one that exceeds the budget runs alone.  The results are the same whatever the grouping.
+ *  - Input and output are HOST bytes; the call returns when every output is complete.  It runs on the calling thread's
+ *    codec for the current device and may be interleaved on one thread with the other transcode and decode calls.
+ *  - A repeated call of the same or a smaller shape makes no heap call. */
+typedef struct uhdr_b200_transcode_file {
+  const void* data;                   /* one JPEG/R file, host memory */
+  size_t size;
+  uhdr_b200_transcode_rung_t* rungs;  /* this file's outputs, as in uhdr_b200_transcode_ladder */
+  int n;                              /* 1..16 */
+  int status;                         /* out: what uhdr_b200_transcode_ladder returns for this file alone */
+} uhdr_b200_transcode_file_t;
+UHDR_EXTERN int uhdr_b200_transcode_ladders(uhdr_b200_transcode_file_t* files, int n);
 
 /* Measurement hooks.  Kernel timing brackets every kernel launch with CUDA events on the
  * launching stream and accumulates per-kernel totals ("name count total_ms min_ms max_ms" lines).

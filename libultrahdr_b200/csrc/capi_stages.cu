@@ -390,16 +390,19 @@ Item* batch_items(int n) {
   return its.data();
 }
 
+// the batched calls' scratch budget per group: 4 GiB, or UHDR_B200_BATCH_GROUP_BYTES
+size_t batch_group_bytes() {
+  size_t group = size_t(4) << 30;
+  if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
+  return group;
+}
+
 // The batched entry points' tail: run(group bytes) unless `rc` (dev_codec's code) already ends the call, that call-level
 // error given to every item without one of its own, each item's status, and the first failing item's code and message
 // ("<what> <index>: ")
 template <class In, class Item, class Run>
 int run_batch(In* items, Item* its, int n, int rc, Run run, const char* what = "item") {
-  if (!rc) {
-    size_t group = size_t(4) << 30;
-    if (const char* e = getenv("UHDR_B200_BATCH_GROUP_BYTES")) group = strtoull(e, nullptr, 10);
-    rc = run(group);
-  }
+  if (!rc) rc = run(batch_group_bytes());
   std::string call_err = rc ? last_error() : "";
   int first = -1;
   for (int i = 0; i < n; i++) {
@@ -636,49 +639,113 @@ UHDR_API int uhdr_b200_transcode_batch(uhdr_b200_transcode_item_t* items, int n,
   return rc;
 }
 
-UHDR_API int uhdr_b200_transcode_ladder(const void* data, size_t size, uhdr_b200_transcode_rung_t* rungs, int n) {
+namespace {
+// uhdr_b200_transcode_ladder's argument checks of the file, which touch no rung
+int ladder_args(const void* data, const uhdr_b200_transcode_rung_t* rungs, int n) {
   if (!data) return fail(E_INVALID_PARAM, "received nullptr for compressed img->data field");
   if (!rungs) return fail(E_INVALID_PARAM, "received nullptr for the rungs");
   if (n < 1 || n > kLadderMaxRungs) return fail(E_INVALID_PARAM, "received %d rungs, expects 1 to %d", n, kLadderMaxRungs);
-  TranscodeBatchItem* its = batch_items<TranscodeBatchItem>(n);
-  bool any = false;
+  return E_OK;
+}
+
+// Both ladder entry points: per file its argument checks (its status, no rung touched), then per rung
+// uhdr_b200_transcode's argument checks in its order, then the file's probe (host only), whose error goes to every rung
+// still valid; the device work when some rung is valid; the call-level error given to every rung without one of its
+// own; each rung's status and out_size, and each file's status: what uhdr_b200_transcode_ladder returns for it alone.
+// The return value is the first failing file's status, and the last error its message, named "file <i>: " when
+// `name_files`.
+int run_ladders(uhdr_b200_transcode_file_t* files, int n, bool name_files) {
+  LadderFile* lf = batch_items<LadderFile>(n);
+  int nr = 0;
   for (int i = 0; i < n; i++) {
-    const uhdr_b200_transcode_rung_t& in = rungs[i];
-    const uhdr_b200_transcode_config_t& cfg = in.cfg;
-    TranscodeBatchItem& b = its[i];
-    b.data = (const uint8_t*)data;
-    b.size = size;
-    b.cfg = cfg;
-    b.out = (uint8_t*)in.out;
-    b.cap = in.cap;
-    b.out_size = 0;
-    // uhdr_b200_transcode's argument checks, in its order
-    b.rc = !in.out ? fail(E_INVALID_PARAM, "received nullptr for the output buffer")
-           : !valid_scale(cfg.k) ? fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", cfg.k)
-           : cfg.base_quality < 0 || cfg.base_quality > 100 || cfg.gainmap_quality < 0 || cfg.gainmap_quality > 100
-               ? fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", cfg.base_quality,
-                      cfg.gainmap_quality)
-               : E_OK;
-    if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
-    any |= !b.rc;
+    const uhdr_b200_transcode_file_t& in = files[i];
+    lf[i].rc = ladder_args(in.data, in.rungs, in.n);
+    if (lf[i].rc) snprintf(lf[i].err, sizeof lf[i].err, "%s", last_error());
+    lf[i].r0 = nr;
+    lf[i].nr = lf[i].rc ? 0 : in.n;
+    nr += lf[i].nr;
   }
-  // then the file's probe, host only: its error goes to every rung still valid
-  DecodedInfo info;
-  if (any) {
-    if (const int prc = JpegRCodec().probe((const uint8_t*)data, size, &info)) {
-      const std::string msg = last_error();
-      for (int i = 0; i < n; i++)
-        if (!its[i].rc) batch_fail(its[i], prc, msg.c_str());
-      any = false;
+  TranscodeBatchItem* its = batch_items<TranscodeBatchItem>(nr);
+  bool any = false;
+  for (int f = 0; f < n; f++) {
+    LadderFile& F = lf[f];
+    if (F.rc) continue;
+    const uhdr_b200_transcode_file_t& in = files[f];
+    F.data = (const uint8_t*)in.data;
+    bool valid = false;
+    for (int i = 0; i < F.nr; i++) {
+      const uhdr_b200_transcode_rung_t& r = in.rungs[i];
+      const uhdr_b200_transcode_config_t& cfg = r.cfg;
+      TranscodeBatchItem& b = its[F.r0 + i];
+      b.data = F.data;
+      b.size = in.size;
+      b.cfg = cfg;
+      b.out = (uint8_t*)r.out;
+      b.cap = r.cap;
+      b.out_size = 0;
+      // uhdr_b200_transcode's argument checks, in its order
+      b.rc = !r.out ? fail(E_INVALID_PARAM, "received nullptr for the output buffer")
+             : !valid_scale(cfg.k) ? fail(E_INVALID_PARAM, "scale denominator %d, expects 1, 2, 4 or 8", cfg.k)
+             : cfg.base_quality < 0 || cfg.base_quality > 100 || cfg.gainmap_quality < 0 || cfg.gainmap_quality > 100
+                 ? fail(E_INVALID_PARAM, "invalid quality factor %d / %d, expects in range [0-100]", cfg.base_quality,
+                        cfg.gainmap_quality)
+                 : E_OK;
+      if (b.rc) snprintf(b.err, sizeof b.err, "%s", last_error());
+      valid |= !b.rc;
     }
+    F.info = DecodedInfo();
+    if (valid) {
+      if (const int prc = JpegRCodec().probe(F.data, in.size, &F.info)) {
+        for (int i = 0; i < F.nr; i++)
+          if (!its[F.r0 + i].rc) batch_fail(its[F.r0 + i], prc, last_error());
+        valid = false;
+      }
+    }
+    for (int i = 0; i < F.nr; i++) its[F.r0 + i].info = F.info;
+    any |= valid;
   }
-  for (int i = 0; i < n; i++) its[i].info = info;
   JpegRCodec* c = nullptr;
-  const int rc = run_batch(rungs, its, n, any ? dev_codec(&c) : E_OK, [&](size_t) {
-    return any ? c->transcode_ladder((const uint8_t*)data, info, its, n) : E_OK;
-  }, "rung");
-  for (int i = 0; i < n; i++) rungs[i].out_size = !its[i].rc || its[i].rc == E_MEM ? its[i].out_size : 0;
-  return rc;
+  int rc = any ? dev_codec(&c) : E_OK;
+  if (!rc && any) rc = c->transcode_ladders(lf, n, its, batch_group_bytes());
+  const std::string call_err = rc ? last_error() : "";
+  int first = -1;
+  for (int f = 0; f < n; f++) {
+    LadderFile& F = lf[f];
+    if (F.rc) {
+      files[f].status = F.rc;
+      if (first < 0) first = f;
+      continue;
+    }
+    int fr = -1;
+    for (int i = 0; i < F.nr; i++) {
+      TranscodeBatchItem& b = its[F.r0 + i];
+      if (rc && !b.rc) batch_fail(b, rc, call_err.c_str());
+      uhdr_b200_transcode_rung_t& r = files[f].rungs[i];
+      r.status = b.rc;
+      // out_size: bytes written, or with UHDR_CODEC_MEM_ERROR the size needed (0 when the file was not assembled)
+      r.out_size = !b.rc || b.rc == E_MEM ? b.out_size : 0;
+      if (b.rc && fr < 0) fr = i;
+    }
+    files[f].status = fr < 0 ? E_OK : its[F.r0 + fr].rc;
+    if (fr >= 0) snprintf(F.err, sizeof F.err, "rung %d: %s", fr, its[F.r0 + fr].err);
+    if (fr >= 0 && first < 0) first = f;
+  }
+  if (first < 0) return E_OK;
+  if (name_files) return fail(files[first].status, "file %d: %s", first, lf[first].err);
+  return fail(files[first].status, "%s", lf[first].err);
+}
+}  // namespace
+
+UHDR_API int uhdr_b200_transcode_ladder(const void* data, size_t size, uhdr_b200_transcode_rung_t* rungs, int n) {
+  if (int rc = ladder_args(data, rungs, n)) return rc;
+  uhdr_b200_transcode_file_t f{data, size, rungs, n, 0};
+  return run_ladders(&f, 1, false);
+}
+
+UHDR_API int uhdr_b200_transcode_ladders(uhdr_b200_transcode_file_t* files, int n) {
+  if (!files) return fail(E_INVALID_PARAM, "received nullptr for the files");
+  if (n < 1) return fail(E_INVALID_PARAM, "received %d files, expects at least 1", n);
+  return run_ladders(files, n, true);
 }
 
 UHDR_API int uhdr_b200_jpeg_encode_dev(const uhdr_raw_image_t* img, int quality, const void* icc, size_t icc_size, void* out,

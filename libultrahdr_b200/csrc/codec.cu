@@ -888,121 +888,136 @@ int JpegRCodec::decode_batch_files(Item* items, int n, int k, int sdr_mode, bool
 }
 template int JpegRCodec::decode_batch_files(TranscodeBatchItem*, int, int, int, bool, int);   // transcode.cu
 
-int JpegRCodec::decode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n) {
-  // one distinct k of the ladder: both JPEGs' plans at 1/k, and the code transcode() gives at that k once decoded
-  struct LadderK {
-    int k, rc, map_rc;
-    char err[256], map_err[256];
-    JpegDecodeJob pj, gj;
-    DevImage sdr, map;
-  } ks[4];
-  int nk = 0;
-  for (int i = 0; i < n; i++) {
-    if (rungs[i].rc) continue;
-    int j = 0;
-    while (j < nk && ks[j].k != rungs[i].cfg.k) j++;
-    if (j == nk) ks[nk++].k = rungs[i].cfg.k;
-  }
-  if (!nk) return E_OK;
-  // 1. both headers once (probe() has read and checked them), then per k the plans in decode_pair's order: the primary,
-  // then the map -- whose error transcode() meets only after the primary's entropy decoding and tail stage
-  const uint8_t* pd = data + info.base_off;
-  const uint8_t* gd = data + info.gainmap_off;
-  JpegHeader ph, gh;
-  int rc = jpeg_read_header(pd, info.base_len, &ph);
-  if (!rc) rc = validate_header(ph);
-  if (rc) {
-    for (int i = 0; i < n; i++)
-      if (!rungs[i].rc) batch_fail(rungs[i], rc, last_error());
-    return E_OK;
-  }
-  int grc = jpeg_read_header(gd, info.gainmap_len, &gh);
-  if (!grc) grc = validate_header(gh);
-  char gerr[256];
-  snprintf(gerr, sizeof gerr, "%s", grc ? last_error() : "");
-  bool need_p = false, need_g = false;
-  for (int j = 0; j < nk; j++) {
-    LadderK& K = ks[j];
-    K.map_rc = E_OK;
-    K.rc = decode_jpeg_plan(ws_, ph, 0, K.k, &K.sdr, &K.pj);
-    if (K.rc == E_MEM) return E_MEM;
-    if (K.rc) {
-      snprintf(K.err, sizeof K.err, "%s", last_error());
-      continue;
-    }
-    need_p = true;
-    K.map_rc = grc ? grc : decode_jpeg_plan(ws_, gh, 0, K.k, &K.map, &K.gj);
-    if (K.map_rc == E_MEM) return E_MEM;
-    if (K.map_rc) snprintf(K.map_err, sizeof K.map_err, "%s", grc ? gerr : last_error());
-    else need_g = true;
-  }
-  // 2. one entropy decoding of each scan some k needs (a scan the device decoder declines goes to the host decoder)
-  if ((int)batch_scans_.size() < 2) batch_scans_.resize(2);
+int JpegRCodec::decode_ladders(LadderFile* files, int n, TranscodeBatchItem* rungs) {
+  if ((int)batch_scans_.size() < 2 * n) batch_scans_.resize(2 * n);
   JpegScanJob* scans = batch_scans_.data();
   int ns = 0;
-  if (need_p) scans[ns++] = JpegScanJob{pd, info.base_len, &ph, {}, 0, {0}};
-  if (need_g) scans[ns++] = JpegScanJob{gd, info.gainmap_len, &gh, {}, 0, {0}};
+  // 1. per file: the distinct k of its valid rungs, both headers once (probe() has read and checked them), then per k
+  // the plans in decode_pair's order: the primary, then the map -- whose error transcode() meets only after the
+  // primary's entropy decoding and tail stage
+  for (int fi = 0; fi < n; fi++) {
+    LadderFile& F = files[fi];
+    TranscodeBatchItem* rs = rungs + F.r0;
+    F.nk = 0;
+    F.ps = F.gs = -1;
+    if (F.rc) continue;
+    for (int i = 0; i < F.nr; i++) {
+      if (rs[i].rc) continue;
+      int j = 0;
+      while (j < F.nk && F.ks[j].k != rs[i].cfg.k) j++;
+      if (j == F.nk) F.ks[F.nk++].k = rs[i].cfg.k;
+    }
+    if (!F.nk) continue;
+    const uint8_t* pd = F.data + F.info.base_off;
+    const uint8_t* gd = F.data + F.info.gainmap_off;
+    int rc = jpeg_read_header(pd, F.info.base_len, &F.ph);
+    if (!rc) rc = validate_header(F.ph);
+    if (rc) {
+      for (int i = 0; i < F.nr; i++)
+        if (!rs[i].rc) batch_fail(rs[i], rc, last_error());
+      F.nk = 0;
+      continue;
+    }
+    int grc = jpeg_read_header(gd, F.info.gainmap_len, &F.gh);
+    if (!grc) grc = validate_header(F.gh);
+    char gerr[256];
+    snprintf(gerr, sizeof gerr, "%s", grc ? last_error() : "");
+    bool need_p = false, need_g = false;
+    for (int j = 0; j < F.nk; j++) {
+      LadderFile::K& K = F.ks[j];
+      K.map_rc = E_OK;
+      K.rc = decode_jpeg_plan(ws_, F.ph, 0, K.k, &K.sdr, &K.pj);
+      if (K.rc == E_MEM) return E_MEM;
+      if (K.rc) {
+        snprintf(K.err, sizeof K.err, "%s", last_error());
+        continue;
+      }
+      need_p = true;
+      K.map_rc = grc ? grc : decode_jpeg_plan(ws_, F.gh, 0, K.k, &K.map, &K.gj);
+      if (K.map_rc == E_MEM) return E_MEM;
+      if (K.map_rc) snprintf(K.map_err, sizeof K.map_err, "%s", grc ? gerr : last_error());
+      else need_g = true;
+    }
+    if (need_p) {
+      F.ps = ns;
+      scans[ns++] = JpegScanJob{pd, F.info.base_len, &F.ph, {}, 0, {0}};
+    }
+    if (need_g) {
+      F.gs = ns;
+      scans[ns++] = JpegScanJob{gd, F.info.gainmap_len, &F.gh, {}, 0, {0}};
+    }
+  }
+  // 2. one entropy decoding of every scan some k of some file needs (a scan the device decoder declines goes to the host
+  // decoder)
+  int rc = E_OK;
   if (ns && (rc = jpeg_entropy_decode_dev(ws_, scans, ns))) return rc;
-  const JpegScanJob* ps = &scans[0];
-  const JpegScanJob* gs = need_g ? &scans[1] : nullptr;
-  // 3. per k in transcode()'s order: the primary's scan and tail stage, the map's plan, scan and tail stage (mode 0
-  // launches nothing there); then one k_idct<0> over both JPEGs at every k left
-  auto fail_k = [](LadderK& K, int r, const char* msg) {
+  // 3. per file and k in transcode()'s order: the primary's scan and tail stage, the map's plan, scan and tail stage
+  // (mode 0 launches nothing there); then one k_idct<0> over both JPEGs of every file at every k left
+  auto fail_k = [](LadderFile::K& K, int r, const char* msg) {
     K.rc = r;
     snprintf(K.err, sizeof K.err, "%s", msg);
   };
-  for (int j = 0; j < nk; j++) {
-    LadderK& K = ks[j];
-    if (K.rc) continue;
-    int r = E_OK;
-    if (ps->rc) {
-      fail_k(K, ps->rc, ps->err);
-    } else if ((r = decode_jpeg_end(ws_, &ph, K.pj, &K.sdr, nullptr))) {
-      if (r == E_MEM) return r;
-      fail_k(K, r, last_error());
-    } else if (K.map_rc) {
-      fail_k(K, K.map_rc, K.map_err);
-    } else if (gs->rc) {
-      fail_k(K, gs->rc, gs->err);
-    } else if ((r = decode_jpeg_end(ws_, &gh, K.gj, &K.map, nullptr))) {
-      if (r == E_MEM) return r;
-      fail_k(K, r, last_error());
-    }
-  }
-  IdctPlane* pl = jpeg_idct_stage(ws_, 6);
+  IdctPlane* pl = jpeg_idct_stage(ws_, 6 * n);
   if (!pl) return E_MEM;
   int np = 0;
-  for (int m = 0; m < 2; m++) {
-    const JpegFrame& f = (m ? gh : ph).frame;
-    const JpegScanJob* sc = m ? gs : ps;   // read only for a k that is left, whose scans were decoded
-    for (int c = 0; c < f.ncomp; c++) {
-      IdctPlane& P = pl[np];
-      P.nout = 0;
-      for (int j = 0; j < nk; j++) {
-        const LadderK& K = ks[j];
-        if (K.rc) continue;
-        const JpegDecodeJob& job = m ? K.gj : K.pj;
-        jpeg_idct_plane(&P, f, c, sc->d_coefs[c], K.k == 1 ? 8 : job.g.s[c], job.planes[c], job.strides[c]);
+  for (int fi = 0; fi < n; fi++) {
+    LadderFile& F = files[fi];
+    const JpegScanJob* ps = F.ps >= 0 ? &scans[F.ps] : nullptr;
+    const JpegScanJob* gs = F.gs >= 0 ? &scans[F.gs] : nullptr;
+    for (int j = 0; j < F.nk; j++) {
+      LadderFile::K& K = F.ks[j];
+      if (K.rc) continue;
+      int r = E_OK;
+      if (ps->rc) {
+        fail_k(K, ps->rc, ps->err);
+      } else if ((r = decode_jpeg_end(ws_, &F.ph, K.pj, &K.sdr, nullptr))) {
+        if (r == E_MEM) return r;
+        fail_k(K, r, last_error());
+      } else if (K.map_rc) {
+        fail_k(K, K.map_rc, K.map_err);
+      } else if (gs->rc) {
+        fail_k(K, gs->rc, gs->err);
+      } else if ((r = decode_jpeg_end(ws_, &F.gh, K.gj, &K.map, nullptr))) {
+        if (r == E_MEM) return r;
+        fail_k(K, r, last_error());
       }
-      if (!P.nout) break;   // no k is left
-      np++;
+    }
+    for (int m = 0; m < 2 && F.nk; m++) {
+      const JpegFrame& f = (m ? F.gh : F.ph).frame;
+      const JpegScanJob* sc = m ? gs : ps;   // read only for a k that is left, whose scans were decoded
+      for (int c = 0; c < f.ncomp; c++) {
+        IdctPlane& P = pl[np];
+        P.nout = 0;
+        for (int j = 0; j < F.nk; j++) {
+          const LadderFile::K& K = F.ks[j];
+          if (K.rc) continue;
+          const JpegDecodeJob& job = m ? K.gj : K.pj;
+          jpeg_idct_plane(&P, f, c, sc->d_coefs[c], K.k == 1 ? 8 : job.g.s[c], job.planes[c], job.strides[c]);
+        }
+        if (!P.nout) break;   // no k is left
+        np++;
+      }
     }
   }
   if (np && (rc = jpeg_idct_multi_dev(ws_, pl, np))) return rc;
   // 4. every rung: its k's code, or that k's decoded pair
-  for (int i = 0; i < n; i++) {
-    TranscodeBatchItem& r = rungs[i];
-    if (r.rc) continue;
-    int j = 0;
-    while (ks[j].k != r.cfg.k) j++;
-    if (ks[j].rc) {
-      batch_fail(r, ks[j].rc, ks[j].err);
-      continue;
+  for (int fi = 0; fi < n; fi++) {
+    LadderFile& F = files[fi];
+    TranscodeBatchItem* rs = rungs + F.r0;
+    for (int i = 0; i < F.nr && F.nk; i++) {
+      TranscodeBatchItem& r = rs[i];
+      if (r.rc) continue;
+      int j = 0;
+      while (F.ks[j].k != r.cfg.k) j++;
+      if (F.ks[j].rc) {
+        batch_fail(r, F.ks[j].rc, F.ks[j].err);
+        continue;
+      }
+      r.ph = F.ph;
+      r.gh = F.gh;
+      r.sdr = F.ks[j].sdr;
+      r.map = F.ks[j].map;
     }
-    r.ph = ph;
-    r.gh = gh;
-    r.sdr = ks[j].sdr;
-    r.map = ks[j].map;
   }
   return E_OK;
 }

@@ -63,7 +63,7 @@ struct DecodeBatchItem : BatchFile {
   uhdr_gainmap_metadata_t* md_out = nullptr;
 };
 
-// One output of JpegRCodec::transcode_batch (a file) or transcode_ladder (a rung): the transcode() settings and output,
+// One output of JpegRCodec::transcode_batch (a file) or transcode_ladders (a rung): the transcode() settings and output,
 // and the two encodes between their batched stages
 struct TranscodeBatchItem : BatchFile {
   uhdr_b200_transcode_config_t cfg{};
@@ -81,8 +81,29 @@ int decode_jpeg_end(Workspace& ws, const JpegHeader* h, const JpegDecodeJob& j, 
 // decode_jpeg_begin's part after the header: the checks and output planes of a decode at 1/k
 int decode_jpeg_plan(Workspace& ws, const JpegHeader& h, int mode, int k, DevImage* out, JpegDecodeJob* j);
 
-// the most rungs one transcode_ladder call takes: it bounds the host plan and the scratch of one call
+// the most rungs of one file of transcode_ladders, and the most distinct (base_quality, gainmap_quality) pairs of one of
+// its groups: it bounds the host plan of transcode_encode
 constexpr int kLadderMaxRungs = 16;
+
+// One file of JpegRCodec::transcode_ladders.  The caller fills the first group of fields; rc != E_OK on entry (the
+// file's own argument error) skips the file.
+struct LadderFile {
+  const uint8_t* data = nullptr;
+  DecodedInfo info;  // probe() of the file
+  int r0 = 0, nr = 0;   // its rungs: [r0, r0 + nr) of the call's rung array, one file after the other
+  int rc = 0;        // the entry points' own: the file's argument error, or what the ladder returns, with its message
+  char err[300] = {0};
+  // decode_ladders' state: both headers, the scans' indices in the group's entropy decoding (-1: not decoded), and per
+  // distinct k of the valid rungs both JPEGs' plans at 1/k and the code transcode() gives at that k once decoded
+  JpegHeader ph, gh;
+  int ps = -1, gs = -1, nk = 0;
+  struct K {
+    int k, rc, map_rc;
+    char err[256], map_err[256];
+    JpegDecodeJob pj, gj;
+    DevImage sdr, map;
+  } ks[4];
+};
 
 // One parked host thread per codec (spawned on first use, kept until the codec dies): runs the gain-map JPEG of a
 // decode next to the primary one without creating a thread per call.
@@ -183,12 +204,13 @@ class JpegRCodec {
   // and two host waits for the encoder.  Each item gets the bytes, size and code transcode() gives for it alone; a
   // failing item writes nothing.  The return value is an error that ends the whole call (CUDA, memory).
   int transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg, size_t group_bytes);
-  // transcode() of one file (`data`, `info` its probe()) into n <= kLadderMaxRungs outputs, each with its own cfg: both
-  // JPEGs entropy-decoded once, one k_idct<0> launch for every k the rungs ask for, then the batch's encode
-  // (transcode_encode).  rungs[i].rc != E_OK on entry skips the rung.  Each rung gets the bytes, size and code
-  // transcode() gives for its cfg alone; a failing rung writes nothing.  The return value is an error that ends the
-  // whole call (CUDA, memory).
-  int transcode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n);
+  // transcode() of many files, each into up to kLadderMaxRungs outputs with their own cfg (rungs[files[i].r0 + j], data
+  // and info set as the file's): per group of files, both JPEGs of every file entropy-decoded once, one k_idct<0> launch
+  // for every k of every file, then the batch's encode (transcode_encode) over every rung of the group.  Groups close
+  // at `group_bytes` of scratch, 2^29 entropy-coded bytes or kLadderMaxRungs distinct quality pairs.  A rung with
+  // rc != E_OK on entry is skipped.  Each rung gets the bytes, size and code transcode() gives for its cfg alone; a
+  // failing rung writes nothing.  The return value is an error that ends the whole call (CUDA, memory).
+  int transcode_ladders(LadderFile* files, int n, TranscodeBatchItem* rungs, size_t group_bytes);
   ~JpegRCodec();
 
  private:
@@ -227,14 +249,17 @@ class JpegRCodec {
   int decode_batch_files(Item* items, int n, int k, int sdr_mode, bool defer_rgba, int map_mode);
   int decode_batch_group(DecodeBatchItem* items, int n, int k, int out_ct, float max_display_boost, cudaStream_t caller);
   int transcode_batch_group(TranscodeBatchItem* items, int n, const uhdr_b200_transcode_config_t& cfg);
-  // transcode_ladder's decode: the headers once, per distinct k the plans of both JPEGs, one entropy decoding of each
-  // scan, the errors in transcode()'s order per k, one k_idct<0>; then each rung's decoded pair (sdr, map, ph, gh)
-  int decode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n);
+  // transcode_ladders' decode of a group: per file the headers once and per distinct k the plans of both JPEGs, one
+  // entropy decoding of every file's scans, per file and k the errors in transcode()'s order, one k_idct<0> over every
+  // file's planes; then each rung's decoded pair (sdr, map, ph, gh)
+  int decode_ladders(LadderFile* files, int n, TranscodeBatchItem* rungs);
   // Both transcode paths' encode, once every item's pair is decoded: per item its cfg's 4:2:2 check of base_420, one
   // k_stage_batch launch, one k_fdct8_code_batch launch per distinct (base_quality, gainmap_quality) pair (at most
   // kLadderMaxRungs of them), one k_huff_encode_batch, two host waits with k_pack_scans, then per item the scan checks
   // and transcode_finish.  A failing item gets its code; the return value is an error that ends the call.
   int transcode_encode(TranscodeBatchItem* items, int n);
+  // transcode_encode's scratch for one item at 1/k: per JPEG the staged planes, the code-word entries and meta, the scan
+  static size_t encode_bytes(const DecodedInfo& in, int k);
   // transcode()'s last stage, once both scans are on the host: API-4's checks, the heads, EXIF, the container, the cap
   int transcode_finish(const uint8_t* data, const DecodedInfo& probed, const JpegHeader& ph, const JpegHeader& gh,
                        const JpegEncodeJob& base_jpeg, const JpegEncodeJob& gm_jpeg, const uhdr_b200_transcode_config_t& cfg,
@@ -243,10 +268,12 @@ class JpegRCodec {
   // scratch of one file of a batched decode at 1/k (w x h, gw x gh: the 1/k sizes; size: the file's bytes)
   static size_t batch_decode_bytes(int w, int h, int gw, int gh, int k, size_t size);
   // The batches' groups: items [g0, g1) as long as their scratch cost(i, &coded) fits `group_bytes` (at least one item)
-  // and their entropy-coded bytes stay below 2^29, so that every bit position of a group fits 32 bits.  run(g0, g1)
-  // runs each group once the previous one's work is done on the host and the workspace is rewound.
-  template <class Cost, class Run>
-  int for_each_group(int n, size_t group_bytes, Cost cost, Run run) {
+  // and their entropy-coded bytes stay below 2^29, so that every bit position of a group fits 32 bits, and admit(i,
+  // fresh) takes item i into the group being formed (a new one when `fresh`, which it must take).  run(g0, g1) runs
+  // each group once the previous one's work is done on the host and the workspace is rewound.
+  static bool admit_any(int, bool) { return true; }
+  template <class Cost, class Run, class Admit = bool (*)(int, bool)>
+  int for_each_group(int n, size_t group_bytes, Cost cost, Run run, Admit admit = admit_any) {
     int rc = E_OK;
     for (int g0 = 0; g0 < n && !rc;) {
       size_t bytes = 0, coded = 0;
@@ -255,6 +282,7 @@ class JpegRCodec {
         size_t c = 0;
         const size_t b = cost(g1, &c);
         if (g1 > g0 && (bytes + b > group_bytes || coded + c >= (1u << 29))) break;
+        if (!admit(g1, g1 == g0)) break;
         bytes += b;
         coded += c;
       }
@@ -265,7 +293,7 @@ class JpegRCodec {
     }
     return rc;
   }
-  std::vector<JpegScanJob> batch_scans_;   // grow-only scratch of decode_batch and transcode_batch
+  std::vector<JpegScanJob> batch_scans_;   // grow-only scratch of the batched calls
   std::vector<JpegIdctJob> batch_idct_;
   std::vector<JpegEncodeJob*> batch_enc_;
   Workspace ws_;

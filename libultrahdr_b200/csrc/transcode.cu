@@ -311,6 +311,17 @@ int upload_plan(Workspace& ws, const T* h, size_t n, T** d) {
 
 }  // namespace
 
+size_t JpegRCodec::encode_bytes(const DecodedInfo& in, int k) {
+  const size_t w = (in.width + k - 1) / k, h = (in.height + k - 1) / k, gw = (in.gm_width + k - 1) / k,
+               gh = (in.gm_height + k - 1) / k;
+  size_t enc = 0;
+  for (int j = 0; j < 2; j++) {   // per JPEG: staged planes, 256 B of code-word entries and 16 B of meta per block, the scan
+    const size_t pw = j ? gw : w, ph = j ? gh : h, blocks = 3 * ((pw + 15) / 8) * ((ph + 15) / 8);
+    enc += 3 * (pw + 8) * (ph + 16) + blocks * (256 + 16) + pw * ph * 6 + 8192;
+  }
+  return enc;
+}
+
 size_t JpegRCodec::batch_decode_bytes(int w, int h, int gw, int gh, int k, size_t size) {
   // coefficients (128 B per 8x8 block, at most 3 components at full size) and their DC terms, planes, coded bits
   const size_t px = (size_t)w * k * h * k + (size_t)gw * k * gh * k;
@@ -327,12 +338,7 @@ int JpegRCodec::transcode_batch(TranscodeBatchItem* items, int n, const uhdr_b20
     *coded = items[i].size;
     const int w = (in.width + k - 1) / k, h = (in.height + k - 1) / k, gw = (in.gm_width + k - 1) / k,
               gh = (in.gm_height + k - 1) / k;
-    size_t enc = 0;
-    for (int j = 0; j < 2; j++) {   // per JPEG: staged planes, 256 B of code-word entries and 16 B of meta per block, the scan
-      const size_t pw = j ? gw : w, ph = j ? gh : h, blocks = 3 * ((pw + 15) / 8) * ((ph + 15) / 8);
-      enc += 3 * (pw + 8) * (ph + 16) + blocks * (256 + 16) + pw * ph * 6 + 8192;
-    }
-    return batch_decode_bytes(w, h, gw, gh, k, items[i].size) + enc;
+    return batch_decode_bytes(w, h, gw, gh, k, items[i].size) + encode_bytes(in, k);
   };
   rc = for_each_group(n, group_bytes, cost, [&](int g0, int g1) { return transcode_batch_group(items + g0, g1 - g0, cfg); });
   if (rc) mark_in_flight();   // as transcode(): kernels of the group may still run
@@ -347,14 +353,59 @@ int JpegRCodec::transcode_batch_group(TranscodeBatchItem* items, int n, const uh
   return transcode_encode(items, n);
 }
 
-int JpegRCodec::transcode_ladder(const uint8_t* data, const DecodedInfo& info, TranscodeBatchItem* rungs, int n) {
+int JpegRCodec::transcode_ladders(LadderFile* files, int n, TranscodeBatchItem* rungs, size_t group_bytes) {
   int rc = settle();
   if (rc) return rc;
-  ws_.rewind();
   map_pending_ = false;
-  rc = decode_ladder(data, info, rungs, n);
-  if (!rc) rc = transcode_encode(rungs, n);
-  if (rc) mark_in_flight();   // as transcode(): kernels of the call may still run
+  // a file's scratch: its coefficients and full-size planes once, its planes at every other k, each rung's encode
+  auto cost = [&](int i, size_t* coded) {
+    const LadderFile& F = files[i];
+    *coded = 0;
+    if (F.rc) return size_t(0);
+    const DecodedInfo& in = F.info;
+    const size_t size = in.base_len + in.gainmap_len;
+    *coded = size;
+    size_t b = batch_decode_bytes(in.width, in.height, in.gm_width, in.gm_height, 1, size);
+    bool seen[9] = {false};
+    for (int j = 0; j < F.nr; j++) {
+      const TranscodeBatchItem& r = rungs[F.r0 + j];
+      if (r.rc) continue;
+      const int k = r.cfg.k;
+      if (k != 1 && !seen[k]) {
+        const size_t w = (in.width + k - 1) / k, h = (in.height + k - 1) / k, gw = (in.gm_width + k - 1) / k,
+                     gh = (in.gm_height + k - 1) / k;
+        b += 3 * (w * h + gw * gh);
+      }
+      seen[k] = true;
+      b += encode_bytes(in, k);
+    }
+    return b;
+  };
+  // the distinct quality pairs of the group being formed, at most kLadderMaxRungs
+  int pairs[kLadderMaxRungs][2], npairs = 0;
+  auto admit = [&](int i, bool fresh) {
+    if (fresh) npairs = 0;
+    int m = npairs;
+    for (int j = 0; j < files[i].nr && !files[i].rc; j++) {
+      const TranscodeBatchItem& r = rungs[files[i].r0 + j];
+      if (r.rc) continue;
+      int p = 0;
+      while (p < m && (pairs[p][0] != r.cfg.base_quality || pairs[p][1] != r.cfg.gainmap_quality)) p++;
+      if (p < m) continue;
+      if (m == kLadderMaxRungs) return false;   // a file alone has at most kLadderMaxRungs rungs: never when fresh
+      pairs[m][0] = r.cfg.base_quality;
+      pairs[m++][1] = r.cfg.gainmap_quality;
+    }
+    npairs = m;
+    return true;
+  };
+  rc = for_each_group(n, group_bytes, cost, [&](int g0, int g1) {
+    // the group's rungs follow each other in `rungs`; a group of files with argument errors alone has none
+    const int r0 = files[g0].r0, r1 = files[g1 - 1].r0 + files[g1 - 1].nr;
+    int r = decode_ladders(files + g0, g1 - g0, rungs);
+    return r || r1 == r0 ? r : transcode_encode(rungs + r0, r1 - r0);
+  }, admit);
+  if (rc) mark_in_flight();   // as transcode(): kernels of the group may still run
   return rc;
 }
 

@@ -195,6 +195,18 @@ def declare_transcode_ladder(lib):
     return lib
 
 
+class TranscodeFile(C.Structure):
+    """uhdr_b200_transcode_file_t: one file of uhdr_b200_transcode_ladders, with its own ladder"""
+    _fields_ = [("data", C.c_void_p), ("size", C.c_size_t), ("rungs", C.POINTER(TranscodeRung)), ("n", C.c_int),
+                ("status", C.c_int)]
+
+
+def declare_transcode_ladders(lib):
+    """argument types of uhdr_b200_transcode_ladders (include/uhdr_b200.h) on a loaded libuhdr_b200"""
+    lib.uhdr_b200_transcode_ladders.argtypes = [C.POINTER(TranscodeFile), C.c_int]
+    return lib
+
+
 def jpeg_encode_batch_stats(lib):
     """-> (k_huff_encode_batch launches, scans they coded) since process start"""
     st = (C.c_ulonglong * 2)()
